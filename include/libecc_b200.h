@@ -223,6 +223,47 @@ int eccb200_ecdsa_verify_msgs_batch(eccb200_ctx *ctx, int hash_type, uint32_t n,
 int eccb200_ecdsa_verify_msgs_batch_dev(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *d_sigs,
 					const uint8_t *d_pubkeys, const uint8_t *d_msgs, const uint64_t *d_offsets,
 					uint8_t *d_digests, int8_t *d_verdict, void *stream);
+/*
+ * Batched Schnorr-family signing of raw messages, hashed on the device.  The hash these schemes sign covers the point
+ * W = k*G, so it runs after the scalar multiplication: k*G (comb), batched normalisation, then one kernel per item that
+ * hashes W with the message and computes s = k + e*x mod q, with e the WHOLE digest reduced mod q:
+ *   ECCB200_ALG_ECSDSA  r = H(W_x || W_y || m), e = OS2I(r) mod q;  sig r || s, hsize + qlen bytes
+ *   ECCB200_ALG_ECOSDSA r = H(W_x || m), e = OS2I(r) mod q;         sig r || s, hsize + qlen bytes
+ *                       (__ecsdsa_sign_init / _finalize, src/sig/ecsdsa_common.c:141-399)
+ *   ECCB200_ALG_ECFSDSA e = H(W_x || W_y || m) mod q;               sig W_x || W_y || s, 2*plen + qlen bytes
+ *                       (src/sig/ecfsdsa.c:120-356)
+ *   ECCB200_ALG_BIP0340 k = H_nonce(t || P_x || m) mod q with t = x' XOR H_aux(a), e = H_challenge(R_x || P_x || m)
+ *                       mod q, x and k negated when y(P) resp. y(R) is odd;  sig R_x || s, plen + qlen bytes
+ *                       (_bip0340_sign, src/sig/bip0340.c:45-101, 161-371)
+ *   privkeys   : n * qlen bytes, x in [1, q-1] (else ECCB200_ERR)
+ *   randomness : n * qlen bytes, what the reference's `rand` callback would return (_ec_sign, src/sig/sig_algs.c:473):
+ *                the nonce k in [1, q-1] (else ECCB200_ERR) for ECSDSA / ECOSDSA / ECFSDSA, the auxiliary value a
+ *                (drawn below 2^(8*qlen), src/sig/bip0340.c:248-254) for BIP0340
+ *   pubkeys    : n * 2*plen affine, BIP0340 only (NULL allowed otherwise): P_x and the parity of P_y are taken from it
+ *                as the reference takes them from the key pair, without checking P = x*G; off the curve: ECCB200_ERR
+ *   msgs / offsets : message i is msgs[offsets[i] .. offsets[i+1]), offsets has n + 1 entries, starts at 0 and never
+ *                decreases (checked here; the _dev form does not re-check it)
+ *   hash_type  : 2 .. 8 (SHA256, SHA384, SHA512, SHA3_224 .. SHA3_512)
+ *   sigs       : [n][siglen], zero unless status is OK
+ *   status     : ECCB200_OK / ECCB200_ERR / ECCB200_RETRY (the reference would fail or restart and fresh randomness
+ *                would succeed: e == 0 or s == 0 for ECSDSA / ECOSDSA, s == 0 for ECFSDSA, a derived k == 0 for BIP0340)
+ * An unsupported sig_type or hash_type returns -1 (eccb200_last_error).  The _dev form follows the rules of every
+ * *_dev entry point (one scratch set per context, calls chained across streams; 16-byte alignment of the privkey,
+ * pubkey, randomness and signature buffers on the 256/384/512-bit curves, not of d_msgs).
+ * NOTE: like every entry point of this library this is a throughput path, NOT a constant-time one.
+ */
+#define ECCB200_ALG_ECSDSA 3
+#define ECCB200_ALG_ECOSDSA 4
+#define ECCB200_ALG_ECFSDSA 5
+#define ECCB200_ALG_BIP0340 20
+int eccb200_schnorr_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+				    const uint8_t *privkeys, const uint8_t *pubkeys, const uint8_t *randomness,
+				    const uint8_t *msgs, const uint64_t *offsets, uint8_t *sigs, int8_t *status);
+int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					const uint8_t *d_privkeys, const uint8_t *d_pubkeys,
+					const uint8_t *d_randomness, const uint8_t *d_msgs,
+					const uint64_t *d_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream);
+
 /* cudaMemcpy device -> host (for callers that do not link the CUDA runtime). */
 int eccb200_copy_to_host(eccb200_ctx *ctx, void *host_dst, const void *d_src, size_t bytes);
 

@@ -41,6 +41,7 @@ ABI_SYMBOLS = [
     "eccb200_fp_addsub_batch", "eccb200_ecdsa_verify_prj_batch", "eccb200_bip0340_verify_batch",
     "eccb200_bip0340_verify_batch_dev", "eccb200_push_results", "eccb200_bind_thread_near_device",
     "eccb200_pipeline_chunk_bounds", "eccb200_double_smul_batch", "eccb200_double_smul_batch_dev",
+    "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev",
 ]
 
 _lib = None
@@ -117,6 +118,10 @@ def load_library() -> ctypes.CDLL:
     lib.eccb200_multi_prj_pt_mul_batch.argtypes = [vp, u64, u8p, u8p, u8p, i8p]
     lib.eccb200_multi_ecdsa_verify_batch.argtypes = [vp, u64, u8p, u8p, u8p, u32, i8p]
     lib.eccb200_ecdsa_verify_msgs_batch_dev.argtypes = [vp, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, i8p, vp]
+    lib.eccb200_schnorr_sign_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp, u8p,
+                                                    i8p]
+    lib.eccb200_schnorr_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp,
+                                                        u8p, i8p, vp]
     lib.eccb200_copy_to_host.argtypes = [vp, vp, vp, ctypes.c_size_t]
     lib.eccb200_bind_thread_near_device.argtypes = [ctypes.c_int]
     lib.eccb200_pipeline_chunk_bounds.argtypes = [u32, u32, u32, u32, ctypes.c_int, vp, ctypes.c_int]
@@ -341,6 +346,41 @@ class Engine:
             self._h, self.HASH_IDS[hash_name], n, d_sigs.data_ptr(), d_pubkeys.data_ptr(), d_msgs.data_ptr(),
             d_offsets.data_ptr(), d_digests.data_ptr(), d_verdict.data_ptr(), ctypes.c_void_p(stream_handle)),
             "eccb200_ecdsa_verify_msgs_batch_dev")
+
+    SCHNORR_ALGS = {"ECSDSA": 3, "ECOSDSA": 4, "ECFSDSA": 5, "BIP0340": 20}  # libecc ec_alg_type values
+
+    def schnorr_sig_len(self, alg: str, hash_name: str) -> int:
+        return {"ECFSDSA": 2 * self.plen + self.qlen, "BIP0340": self.plen + self.qlen}.get(
+            alg, self.HASH_LEN[hash_name] + self.qlen)
+
+    def schnorr_sign_msgs_batch(self, alg: str, hash_name: str, privkeys, randomness, msgs,
+                                pubkeys=None) -> Tuple[np.ndarray, np.ndarray]:
+        """ECSDSA / ECOSDSA / ECFSDSA / BIP0340 signatures of raw messages, hashed on the device.  randomness[i] is what
+        the reference's rand callback would return: the nonce k (qlen bytes) or, for BIP0340, the auxiliary value a.
+        pubkeys (n*2*plen affine) are required for BIP0340 only.  Returns (sigs[n, siglen], status[n]):
+        0 OK, -1 ERR, 2 RETRY (see include/libecc_b200.h)."""
+        n = len(msgs)
+        d = _as_u8(privkeys, n * self.qlen)
+        r = _as_u8(randomness, n * self.qlen)
+        pk = _as_u8(pubkeys, n * 2 * self.plen) if pubkeys is not None else None
+        blob, off = self._pack_msgs(msgs)
+        sigs = np.zeros((n, self.schnorr_sig_len(alg, hash_name)), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_schnorr_sign_msgs_batch(
+            self._h, self.SCHNORR_ALGS[alg], self.HASH_IDS[hash_name], n, d.ctypes.data,
+            pk.ctypes.data if pk is not None else None, r.ctypes.data, blob.ctypes.data, off.ctypes.data,
+            sigs.ctypes.data, status.ctypes.data), "eccb200_schnorr_sign_msgs_batch")
+        return sigs, status
+
+    def schnorr_sign_msgs_batch_dev(self, alg: str, hash_name: str, d_privkeys, d_randomness, d_msgs, d_offsets,
+                                    d_sigs, d_status, d_pubkeys=None, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`); d_offsets: n + 1 uint64 entries, not re-checked."""
+        n = d_privkeys.numel() // self.qlen
+        self._check(self.lib.eccb200_schnorr_sign_msgs_batch_dev(
+            self._h, self.SCHNORR_ALGS[alg], self.HASH_IDS[hash_name], n, d_privkeys.data_ptr(),
+            d_pubkeys.data_ptr() if d_pubkeys is not None else None, d_randomness.data_ptr(), d_msgs.data_ptr(),
+            d_offsets.data_ptr(), d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)),
+            "eccb200_schnorr_sign_msgs_batch_dev")
 
     def copy_to_host(self, d_ptr: int, nbytes: int) -> np.ndarray:
         out = np.empty(nbytes, dtype=np.uint8)

@@ -21,6 +21,7 @@
  */
 #pragma once
 #include "fp.cuh"
+#include "sha2.cuh"
 
 namespace eccb200 {
 
@@ -873,6 +874,132 @@ ECC_HD int bip0340_verify_tail(const Fe<C::N> &r, const Fe<C::N> &s, const Fe<C:
 	if (inf) return 2;
 	if (y.w[0] & 1u) return 3;
 	return F::eq(x, r) ? 0 : 3;
+}
+
+/* ------------------------------------------------------------------ Schnorr-family signing (ECSDSA .. BIP0340) */
+
+/* ec_alg_type values of the reference (lib_ecc_types.h) for the four schemes whose hash covers W = k*G */
+enum { SIG_ECSDSA = 3, SIG_ECOSDSA = 4, SIG_ECFSDSA = 5, SIG_BIP0340 = 20 };
+/* the longest hash prefix: H(tag) || H(tag) || (R_x or t) || P_x with 64-byte digests on the 521-bit curve */
+constexpr int kSchnorrMaxPrefix = 2 * 64 + 2 * 66;
+
+/* r || s: hsize + qlen (ECSDSA / ECOSDSA), 2*plen + qlen (ECFSDSA), plen + qlen (BIP0340) */
+template <class C> ECC_HD int schnorr_sig_len(int sig_type, int digest_size)
+{
+	return sig_type == SIG_ECFSDSA ? 2 * C::PLEN + C::QLEN :
+	       sig_type == SIG_BIP0340 ? C::PLEN + C::QLEN : digest_size + C::QLEN;
+}
+
+/* H(tag) of the three BIP0340 tags (sig/bip0340.c:41-43): 0 aux, 1 nonce, 2 challenge */
+ECC_D void bip0340_tag_hash(int hash_type, int tag, uint8_t *out)
+{
+	const char *s = tag == 0 ? "BIP0340/aux" : (tag == 1 ? "BIP0340/nonce" : "BIP0340/challenge");
+	const uint32_t len = tag == 0 ? 11u : (tag == 1 ? 13u : 17u);
+	hash_src(hash_type, ByteSpan{ (const uint8_t *)s }, len, out);
+}
+
+/*
+ * The BIP0340 nonce (_bip0340_sign, sig/bip0340.c:243-297): d = x, or q - x when y(P) is odd (:237, :74-101);
+ * t = d XOR H_aux(a) and k = H_nonce(t || P_x || m) mod q, with the reference's two branches (:267-280): when
+ * qlen > digest size the first digest-size bytes of d are XORed and qlen bytes hashed, otherwise the first qlen bytes
+ * of H_aux(a) are XORed and digest-size bytes hashed.  H_tag(z) = H(H(tag) || H(tag) || z); tag_aux / tag_nonce are
+ * the H(tag) digests.  x must be in [1, q-1]; P is the affine wire key, a the qlen-byte auxiliary randomness.
+ */
+template <class C>
+ECC_D void bip0340_nonce(Fe<C::N> &k, int hash_type, const Fe<C::N> &x, const uint8_t *P, const uint8_t *aux,
+			 const uint8_t *msg, uint64_t mlen, const uint8_t *tag_aux, const uint8_t *tag_nonce)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int PL = C::PLEN, QL = C::QLEN;
+	const int ds = sha2_digest_size(hash_type);
+	uint8_t pre[kSchnorrMaxPrefix], h[64], db[QL];
+	Fe<C::N> d = x;
+	if (P[2 * PL - 1] & 1u) Fq::neg(d, d);
+	store_be<C::N>(db, d, QL);
+	for (int i = 0; i < ds; i++) pre[i] = pre[ds + i] = tag_aux[i];
+	for (int i = 0; i < QL; i++) pre[2 * ds + i] = aux[i];
+	hash_segments(hash_type, pre, (uint32_t)(2 * ds + QL), nullptr, 0, h); /* H_aux(a) */
+	for (int i = 0; i < ds; i++) pre[i] = pre[ds + i] = tag_nonce[i];
+	int np = 2 * ds;
+	if (QL > ds) {
+		for (int i = 0; i < QL; i++) pre[np + i] = db[i] ^ (i < ds ? h[i] : 0u);
+		np += QL;
+	} else {
+		for (int i = 0; i < ds; i++) pre[np + i] = h[i] ^ (i < QL ? db[i] : 0u);
+		np += ds;
+	}
+	for (int i = 0; i < PL; i++) pre[np + i] = P[i];
+	np += PL;
+	hash_segments(hash_type, pre, (uint32_t)np, msg, mlen, h);
+	digest_full_mod_q<C>(k, h, (uint32_t)ds);
+}
+
+/*
+ * One Schnorr-family signature from W = k*G (affine wire bytes, as K4 writes them), the private scalar x and the
+ * nonce k (plain integers) and the message (in memory, read where it lies):
+ *   ECSDSA  r = H(W_x || W_y || m), e = OS2I(r) mod q   (__ecsdsa_sign_init / _finalize, sig/ecsdsa_common.c:141-399)
+ *   ECOSDSA r = H(W_x || m), e = OS2I(r) mod q
+ *   ECFSDSA r = W_x || W_y, e = H(r || m) mod q          (sig/ecfsdsa.c:120-356)
+ *   BIP0340 r = R_x, e = H_challenge(R_x || P_x || m) mod q, x and k negated when y(P) resp. y(R) is odd
+ *           (sig/bip0340.c:161-371); tag_challenge = H("BIP0340/challenge"), P the affine wire key (key_ok: on the curve)
+ * and s = k + e*x mod q.  e is the WHOLE digest reduced mod q (nn_init_from_buf + nn_mod), not the ECDSA truncation.
+ * Returns 0 (sig written), -1 (x or k outside [1, q-1], or a BIP0340 key off the curve) or 2 (the reference fails or
+ * restarts and fresh randomness would succeed: e == 0 or s == 0 for ECSDSA / ECOSDSA, s == 0 for ECFSDSA, a derived
+ * k == 0 for BIP0340); sig (schnorr_sig_len bytes) is zero unless 0 is returned.
+ */
+template <class C>
+ECC_D int schnorr_sign_core(uint8_t *sig, int sig_type, int hash_type, const uint8_t *W, const Fe<C::N> &x,
+			    const Fe<C::N> &k, const uint8_t *msg, uint64_t mlen, const uint8_t *P, bool key_ok,
+			    const uint8_t *tag_challenge)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, PL = C::PLEN, QL = C::QLEN;
+	const int ds = sha2_digest_size(hash_type);
+	const int siglen = schnorr_sig_len<C>(sig_type, ds);
+	const bool bip = sig_type == SIG_BIP0340;
+	int st = 0;
+	if (!key_ok || Fq::is_zero(x) || Fq::geq_mod(x)) st = -1;
+	else if (Fq::is_zero(k) || Fq::geq_mod(k)) st = bip ? 2 : -1; /* BIP0340: k is derived, reduced mod q */
+	if (st != 0) {
+		for (int i = 0; i < siglen; i++) sig[i] = 0;
+		return st;
+	}
+	uint8_t pre[kSchnorrMaxPrefix], h[64];
+	int np = 0;
+	if (bip)
+		for (int i = 0; i < ds; i++) pre[i] = pre[ds + i] = tag_challenge[i];
+	np = bip ? 2 * ds : 0;
+	for (int i = 0; i < PL; i++) pre[np + i] = W[i];
+	np += PL;
+	if (sig_type == SIG_ECSDSA || sig_type == SIG_ECFSDSA) {
+		for (int i = 0; i < PL; i++) pre[np + i] = W[PL + i];
+		np += PL;
+	} else if (bip) {
+		for (int i = 0; i < PL; i++) pre[np + i] = P[i];
+		np += PL;
+	}
+	hash_segments(hash_type, pre, (uint32_t)np, msg, mlen, h);
+	Fe<N> e, xx = x, kk = k, xm, t, s;
+	digest_full_mod_q<C>(e, h, (uint32_t)ds);
+	if (bip) {
+		if (P[2 * PL - 1] & 1u) Fq::neg(xx, xx);
+		if (W[2 * PL - 1] & 1u) Fq::neg(kk, kk);
+	}
+	Fq::to_mont(xm, xx);
+	Fq::mul(t, e, xm); /* e*x mod q (plain: one factor in the Montgomery domain) */
+	Fq::add(s, kk, t);
+	bool retry = (!bip && Fq::is_zero(s)) || ((sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA) && Fq::is_zero(e));
+	if (retry) {
+		for (int i = 0; i < siglen; i++) sig[i] = 0;
+		return 2;
+	}
+	const int rlen = siglen - QL;
+	if (sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA)
+		for (int i = 0; i < rlen; i++) sig[i] = h[i];
+	else
+		for (int i = 0; i < rlen; i++) sig[i] = W[i];
+	store_be<N>(sig + rlen, s, QL);
+	return 0;
 }
 
 /* r, s in [1, q-1]?  (__ecdsa_verify_init, sig/ecdsa_common.c:653-658) */

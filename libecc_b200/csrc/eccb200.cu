@@ -87,6 +87,8 @@ struct eccb200_ctx {
 	uint8_t *unique_io = nullptr; /* device buffer of eccb200_prj_pt_unique_batch (in || out || status), grown on demand:
 	                               * a cudaMalloc / cudaFree pair per call cost up to a second on a busy allocator */
 	size_t unique_io_bytes = 0;
+	uint8_t *sign_k = nullptr; /* [sign_k_cap][qlen] BIP0340 nonces of the device-pointer Schnorr signer, grown on demand */
+	uint32_t sign_k_cap = 0;
 	/* optional per-kernel timing of the device-pointer API (bench.py's roofline leg) */
 	bool profiling = false;
 	static const int kProfCalls = 64;
@@ -321,6 +323,7 @@ extern "C" void eccb200_ctx_destroy(eccb200_ctx *ctx)
 	msm_release(ctx);
 	if (ctx->msm_in) cudaFree(ctx->msm_in);
 	if (ctx->unique_io) cudaFree(ctx->unique_io);
+	if (ctx->sign_k) cudaFree(ctx->sign_k);
 	if (ctx->table) cudaFree(ctx->table);
 	if (ctx->jac) cudaFree(ctx->jac);
 	if (ctx->prefix) cudaFree(ctx->prefix);
@@ -1613,6 +1616,139 @@ extern "C" int eccb200_ecdsa_verify_msgs_batch_dev(eccb200_ctx *ctx, int hash_ty
 	CUDA_OK(cudaSetDevice(ctx->device));
 	if (hash_dev(ctx, hash_type, n, d_msgs, d_offsets, d_digests, (cudaStream_t)stream)) return -1;
 	return verify_dev(ctx, n, d_sigs, d_pubkeys, d_digests, (uint32_t)ds, d_verdict, (cudaStream_t)stream);
+}
+
+/* ------------------------------------------------------------------------------------------ Schnorr-family sign */
+
+static const char *kSchnorrAlgMsg = "unsupported sig_type (ECSDSA = 3, ECOSDSA = 4, ECFSDSA = 5, BIP0340 = 20)";
+static bool schnorr_alg_ok(int sig_type)
+{
+	return sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA || sig_type == SIG_ECFSDSA || sig_type == SIG_BIP0340;
+}
+
+/* BIP0340 nonce kernel (k into k_buf), K1 on k (or on the caller's nonces), K4, finish kernel — all on `st` */
+static int schnorr_sign_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *d_priv,
+			    const uint8_t *d_pub, const uint8_t *d_rand, const uint8_t *d_msgs, const uint64_t *d_off,
+			    uint8_t *d_sigs, int8_t *d_status, uint32_t *jac, uint32_t *prefix, uint8_t *aff, uint8_t *k_buf,
+			    cudaStream_t st)
+{
+	if (n == 0) return 0;
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		const uint8_t *d_k = d_rand;
+		if (sig_type == SIG_BIP0340) {
+			LaunchMisc<C>::bip0340_nonce(n, hash_type, d_priv, d_pub, d_rand, d_msgs, d_off, k_buf, st);
+			d_k = k_buf;
+			ctx->launches += 1;
+		}
+		LaunchFixed<C>::fixed(n, d_k, ctx->table, ctx->w, jac, d_status, st);         /* W = k*G   */
+		LaunchMisc<C>::to_affine(affine_grid(ctx, n), n, jac, prefix, aff, d_status, st); /* affine W  */
+		LaunchMisc<C>::schnorr_finish(n, sig_type, hash_type, d_priv, d_pub, d_k, d_msgs, d_off, aff, d_sigs,
+					      d_status, st);                                   /* hash, s   */
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 3;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+extern "C" int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+						   const uint8_t *d_privkeys, const uint8_t *d_pubkeys,
+						   const uint8_t *d_randomness, const uint8_t *d_msgs,
+						   const uint64_t *d_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream)
+{
+	if (!ctx) return fail("null argument");
+	if (!schnorr_alg_ok(sig_type)) return fail(kSchnorrAlgMsg);
+	if (!sha2_digest_size(hash_type)) return fail("unsupported hash (SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224..512 = 5..8)");
+	if (n && (!d_privkeys || !d_randomness || !d_offsets || !d_sigs || !d_status ||
+		  (sig_type == SIG_BIP0340 && !d_pubkeys)))
+		return fail("null argument");
+	if (misaligned16(ctx, { d_privkeys, d_pubkeys, d_randomness, d_sigs })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_work(ctx, n)) return -1;
+	if (sig_type == SIG_BIP0340 && ctx->sign_k_cap < n) {
+		CUDA_OK(cudaDeviceSynchronize()); /* an earlier call may still read the buffer that is about to be replaced */
+		if (ctx->sign_k) cudaFree(ctx->sign_k);
+		ctx->sign_k = nullptr;
+		ctx->sign_k_cap = 0;
+		CUDA_OK(cudaMalloc(&ctx->sign_k, (size_t)n * ctx->qlen));
+		ctx->sign_k_cap = n;
+	}
+	return schnorr_sign_dev(ctx, sig_type, hash_type, n, d_privkeys, d_pubkeys, d_randomness, d_msgs, d_offsets, d_sigs,
+				d_status, ctx->jac, ctx->prefix, ctx->aff, ctx->sign_k, (cudaStream_t)stream);
+}
+
+/* Host-pointer form: chunks of four waves on two streams like eccb200_ecdsa_verify_msgs_batch (a chunk's copies
+ * overlap the other chunk's kernels), K1 / K4 scratch from the per-stream stage buffers, the chunk's message bytes
+ * addressed with the caller's absolute offsets against a shifted base. */
+extern "C" int eccb200_schnorr_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					       const uint8_t *privkeys, const uint8_t *pubkeys, const uint8_t *randomness,
+					       const uint8_t *msgs, const uint64_t *offsets, uint8_t *sigs, int8_t *status)
+{
+	if (!ctx) return fail("null argument");
+	if (!schnorr_alg_ok(sig_type)) return fail(kSchnorrAlgMsg);
+	const int ds = sha2_digest_size(hash_type);
+	if (!ds) return fail("unsupported hash (SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224..512 = 5..8)");
+	const bool bip = sig_type == SIG_BIP0340;
+	if (n && (!privkeys || !randomness || !offsets || !sigs || !status || (bip && !pubkeys))) return fail("null argument");
+	if (n == 0) return 0;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_stages(ctx, 1, 1)) return -1; /* the stage_jac / stage_prefix / stage_aff scratch */
+	const uint32_t step = std::min(ctx->chunk_eq, ctx->chunk);
+	const size_t ql = ctx->qlen, pki = bip ? 2 * (size_t)ctx->plen : 0;
+	size_t siglen = 0;
+	dispatch(ctx->curve_id, [&](auto c) {
+		siglen = (size_t)schnorr_sig_len<decltype(c)>(sig_type, ds);
+		return 0;
+	});
+	size_t max_msg = 0;
+	for (uint32_t lo = 0; lo < n; lo += step) {
+		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n);
+		max_msg = std::max<size_t>(max_msg, (size_t)(offsets[hi] - offsets[lo]));
+	}
+	const uint32_t cap = std::min(step, n);
+	const size_t b_x = align16(cap * ql), b_pk = align16(cap * pki), b_r = align16(cap * ql),
+		     b_k = bip ? align16(cap * ql) : 0, b_msg = align16(max_msg + 16),
+		     b_off = align16(((size_t)cap + 1) * sizeof(uint64_t)), b_sig = align16(cap * siglen), b_st = align16(cap);
+	const size_t stage = b_x + b_pk + b_r + b_k + b_msg + b_off + b_sig + b_st;
+	uint8_t *d = nullptr;
+	CUDA_OK(cudaMalloc(&d, 2 * stage));
+	int rc = 0;
+	uint32_t c = 0;
+	for (uint32_t lo = 0; lo < n && !rc; lo += step, c++) {
+		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n), cnt = hi - lo;
+		const int s = (int)(c & 1);
+		cudaStream_t st = ctx->streams[s];
+		uint8_t *d_x = d + (size_t)s * stage, *d_pk = d_x + b_x, *d_r = d_pk + b_pk, *d_k = d_r + b_r, *d_msg = d_k + b_k,
+			*d_off = d_msg + b_msg, *d_sig = d_off + b_off, *d_st = d_sig + b_sig;
+		const size_t mbytes = (size_t)(offsets[hi] - offsets[lo]);
+		if (cudaMemcpyAsync(d_x, privkeys + lo * ql, cnt * ql, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+		    (bip && cudaMemcpyAsync(d_pk, pubkeys + lo * pki, cnt * pki, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+		    cudaMemcpyAsync(d_r, randomness + lo * ql, cnt * ql, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+		    (mbytes && cudaMemcpyAsync(d_msg, msgs + offsets[lo], mbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
+		    cudaMemcpyAsync(d_off, offsets + lo, ((size_t)cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st) !=
+			    cudaSuccess) {
+			rc = fail("H2D copy failed");
+			break;
+		}
+		/* the kernels add the caller's absolute offsets to this base: the chunk's bytes start at offsets[lo] */
+		rc = schnorr_sign_dev(ctx, sig_type, hash_type, cnt, d_x, bip ? d_pk : nullptr, d_r, d_msg - offsets[lo],
+				      (const uint64_t *)d_off, d_sig, (int8_t *)d_st, ctx->stage_jac[s], ctx->stage_prefix[s],
+				      ctx->stage_aff[s], d_k, st);
+		if (!rc && (cudaMemcpyAsync(sigs + lo * siglen, d_sig, cnt * siglen, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+			    cudaMemcpyAsync(status + lo, d_st, cnt, cudaMemcpyDeviceToHost, st) != cudaSuccess))
+			rc = fail("D2H copy failed");
+	}
+	const std::string keep = g_err;
+	for (int s2 = 0; s2 < 2; s2++)
+		if (cudaStreamSynchronize(ctx->streams[s2]) != cudaSuccess && !rc) rc = fail("stream synchronisation failed");
+	if (rc && !keep.empty()) g_err = keep;
+	cudaFree(d);
+	return rc;
 }
 
 /* cudaMemcpy device -> host for callers that do not link the CUDA runtime (bench.py reads peer-written buffers). */

@@ -1069,6 +1069,74 @@ __global__ void __launch_bounds__(128) k_ecdsa_sign_finish(uint32_t n, const uin
 	}
 }
 
+/* ------------------------------------------------------------------------------------------ Schnorr-family sign */
+
+/* H(tag) of BIP0340 tags tag0 .. tag0 + ntags - 1 into shared memory, one thread per tag: once per CTA, not per item */
+__device__ __forceinline__ void bip0340_tags_shared(uint8_t (*tags)[64], int hash_type, int tag0, int ntags)
+{
+	if ((int)threadIdx.x < ntags) bip0340_tag_hash(hash_type, tag0 + (int)threadIdx.x, tags[threadIdx.x]);
+	__syncthreads();
+}
+
+/* BIP0340 nonces before K1: k[i] = H_nonce(t || P_x || m) mod q (bip0340_nonce), or 0 when x is outside [1, q-1] or
+ * the key is not on the curve (the finish kernel tells those apart from a derived k == 0).  Messages as
+ * k_sha2_batch: message i is msgs[off[i] .. off[i+1]). */
+template <class C>
+__global__ void __launch_bounds__(128) k_bip0340_nonce(uint32_t n, int hash_type, const uint8_t *__restrict__ privkeys,
+						       const uint8_t *__restrict__ pubkeys, const uint8_t *__restrict__ aux,
+						       const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+						       uint8_t *__restrict__ k_out)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N;
+	__shared__ uint8_t tags[2][64];
+	bip0340_tags_shared(tags, hash_type, 0, 2);
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	Fe<N> x, k;
+	Aff<C> P;
+	load_wire<N, C::QLEN>(x, privkeys + (size_t)idx * C::QLEN);
+	const uint8_t *pk = pubkeys + (size_t)idx * (2 * C::PLEN);
+	Fq::set_zero(k);
+	if (load_affine_checked<C>(P, pk) && !Fq::is_zero(x) && !Fq::geq_mod(x))
+		bip0340_nonce<C>(k, hash_type, x, pk, aux + (size_t)idx * C::QLEN, msgs + off[idx], off[idx + 1] - off[idx],
+				 tags[0], tags[1]);
+	store_wire<N, C::QLEN>(k_out + (size_t)idx * C::QLEN, k);
+}
+
+/* After K1 (k*G) and K4 (affine W): the hash over W and the message, then s = k + e*x mod q (schnorr_sign_core).
+ * sigs: [n][schnorr_sig_len], status: 0 / -1 / 2 (ECCB200_OK / _ERR / _RETRY). */
+template <class C>
+__global__ void __launch_bounds__(128) k_schnorr_sign_finish(uint32_t n, int sig_type, int hash_type,
+							     const uint8_t *__restrict__ privkeys,
+							     const uint8_t *__restrict__ pubkeys,
+							     const uint8_t *__restrict__ nonces,
+							     const uint8_t *__restrict__ msgs,
+							     const uint64_t *__restrict__ off,
+							     const uint8_t *__restrict__ W_aff, uint8_t *__restrict__ sigs,
+							     int8_t *__restrict__ status)
+{
+	constexpr int N = C::N;
+	const bool bip = sig_type == SIG_BIP0340;
+	__shared__ uint8_t tags[1][64];
+	if (bip) bip0340_tags_shared(tags, hash_type, 2, 1);
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	Fe<N> x, k;
+	load_wire<N, C::QLEN>(x, privkeys + (size_t)idx * C::QLEN);
+	load_wire<N, C::QLEN>(k, nonces + (size_t)idx * C::QLEN);
+	const uint8_t *pk = bip ? pubkeys + (size_t)idx * (2 * C::PLEN) : nullptr;
+	bool key_ok = true;
+	if (bip) {
+		Aff<C> P;
+		key_ok = load_affine_checked<C>(P, pk);
+	}
+	const int siglen = schnorr_sig_len<C>(sig_type, sha2_digest_size(hash_type));
+	status[idx] = (int8_t)schnorr_sign_core<C>(sigs + (size_t)idx * siglen, sig_type, hash_type,
+						   W_aff + (size_t)idx * (2 * C::PLEN), x, k, msgs + off[idx],
+						   off[idx + 1] - off[idx], pk, key_ok, tags[0]);
+}
+
 /* Private-key sanity check of __ecdsa_init_pub_key (sig/ecdsa_common.c:188): x < q, else the key is rejected (-1).
  * Run before K1, which would silently reduce x mod q.  state[i] is only ever lowered to -1. */
 template <class C>
@@ -1289,6 +1357,12 @@ template <class C> struct LaunchMisc {
 	static void sign_finish(uint32_t blocks, uint32_t n, const uint8_t *privkeys, const uint8_t *nonces,
 				const uint8_t *digests, uint32_t hlen, const uint8_t *kG_aff, uint32_t *prefix,
 				uint8_t *sigs, int8_t *status, cudaStream_t st);
+	static void bip0340_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *pubkeys,
+				  const uint8_t *aux, const uint8_t *msgs, const uint64_t *off, uint8_t *k_out,
+				  cudaStream_t st);
+	static void schnorr_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *privkeys,
+				   const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
+				   const uint8_t *W_aff, uint8_t *sigs, int8_t *status, cudaStream_t st);
 	static void fp_mul(int which, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out, cudaStream_t st);
 	static void fp_addsub(int which, int op, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out,
 			      cudaStream_t st);
@@ -1377,6 +1451,21 @@ void LaunchMisc<C>::sign_finish(uint32_t blocks, uint32_t n, const uint8_t *priv
 {
 	k_ecdsa_sign_finish<C><<<blocks, kThreads, 0, st>>>(n, privkeys, nonces, digests, hlen, kG_aff, prefix, sigs,
 							     status);
+}
+template <class C>
+void LaunchMisc<C>::bip0340_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *pubkeys,
+				  const uint8_t *aux, const uint8_t *msgs, const uint64_t *off, uint8_t *k_out,
+				  cudaStream_t st)
+{
+	k_bip0340_nonce<C><<<grid_for(n), kThreads, 0, st>>>(n, hash_type, privkeys, pubkeys, aux, msgs, off, k_out);
+}
+template <class C>
+void LaunchMisc<C>::schnorr_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *privkeys,
+				   const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
+				   const uint8_t *W_aff, uint8_t *sigs, int8_t *status, cudaStream_t st)
+{
+	k_schnorr_sign_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, sig_type, hash_type, privkeys, pubkeys, nonces, msgs,
+								    off, W_aff, sigs, status);
 }
 template <class C>
 void LaunchMisc<C>::prj_unique(uint32_t blocks, uint32_t n, const uint8_t *prj, uint32_t *jac, uint32_t *prefix,

@@ -5,26 +5,54 @@
  * Reference counterparts (relative to /root/reference/src): sha256_init/update/final hash/sha256.c:70,96,145 (scattered
  * form :201), SHA-384/512 hash/sha384.c, hash/sha512.c over hash/sha512_core.c; generic front end hash_mapping
  * hash/hash_algs.h:232-241.  The algorithm is FIPS 180-4; constants come from tools/gen_sha2_constants.py.
+ *
+ * The input is a byte source: one contiguous message (ByteSpan), or a short prefix held by the thread followed by a
+ * message in global memory (Seg2: the Schnorr-family signers hash W || m or H(tag) || H(tag) || ... || m without
+ * building the concatenation).  Plain C++ outside nvcc, so that the host build of the tests runs the same code.
  */
 #pragma once
 #include <stdint.h>
 #include "sha3.cuh"
 
+#if defined(__CUDACC__)
+#define SHA2_D __device__ __forceinline__
+#else
+#define SHA2_D inline
+#endif
+
 namespace eccb200 {
 
+/* internal linkage: every translation unit that hashes gets its own copy of the constants */
+namespace {
+#if defined(__CUDACC__)
 #include "sha2_constants.inc"
+#else
+#define __device__
+#define __constant__
+#include "sha2_constants.inc"
+#undef __device__
+#undef __constant__
+#endif
+} // namespace
 
-__device__ __forceinline__ uint32_t rotr32(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
-__device__ __forceinline__ uint64_t rotr64(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
+SHA2_D uint32_t rotr32(uint32_t x, int n)
+{
+#if defined(__CUDA_ARCH__)
+	return __funnelshift_r(x, x, n);
+#else
+	return (x >> n) | (x << (32 - n));
+#endif
+}
+SHA2_D uint64_t rotr64(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
 
 /* byte i of the padded message: data, then 0x80, then zeros; the caller overrides the trailing length field */
-__device__ __forceinline__ uint32_t padded_byte(const uint8_t *__restrict__ m, uint64_t len, uint64_t i)
+template <class Src> SHA2_D uint32_t padded_byte(const Src &m, uint64_t len, uint64_t i)
 {
-	return (i < len) ? (uint32_t)m[i] : ((i == len) ? 0x80u : 0u);
+	return (i < len) ? m[i] : ((i == len) ? 0x80u : 0u);
 }
 
 /* digest: 32 bytes, big-endian words */
-__device__ inline void sha256_device(const uint8_t *__restrict__ m, uint64_t len, uint8_t *__restrict__ digest)
+template <class Src> SHA2_D void sha256_src(const Src &m, uint64_t len, uint8_t *__restrict__ digest)
 {
 	uint32_t h[8];
 #pragma unroll
@@ -75,8 +103,9 @@ __device__ inline void sha256_device(const uint8_t *__restrict__ m, uint64_t len
 }
 
 /* SHA-512 core with selectable initial value; out_bytes = 48 (SHA-384) or 64 (SHA-512) */
-__device__ inline void sha512_family_device(const uint8_t *__restrict__ m, uint64_t len, uint8_t *__restrict__ digest,
-					    const uint64_t *__restrict__ iv, int out_bytes)
+template <class Src>
+SHA2_D void sha512_family_src(const Src &m, uint64_t len, uint8_t *__restrict__ digest, const uint64_t *__restrict__ iv,
+			      int out_bytes)
 {
 	uint64_t h[8];
 #pragma unroll
@@ -121,17 +150,45 @@ __device__ inline void sha512_family_device(const uint8_t *__restrict__ m, uint6
 	for (int i = 0; i < out_bytes; i++) digest[i] = (uint8_t)(h[i >> 3] >> (8 * (7 - (i & 7))));
 }
 
+SHA2_D void sha256_device(const uint8_t *__restrict__ m, uint64_t len, uint8_t *__restrict__ digest)
+{
+	sha256_src(ByteSpan{ m }, len, digest);
+}
+SHA2_D void sha512_family_device(const uint8_t *__restrict__ m, uint64_t len, uint8_t *__restrict__ digest,
+				 const uint64_t *__restrict__ iv, int out_bytes)
+{
+	sha512_family_src(ByteSpan{ m }, len, digest, iv, out_bytes);
+}
+
 /* hash_alg_type values of the reference (lib_ecc_types.h:82-): SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224 = 5,
  * SHA3_256 = 6, SHA3_384 = 7, SHA3_512 = 8 (sha3.cuh) */
-__host__ __device__ inline int sha2_digest_size(int hash_type)
+SHA3_HD int sha2_digest_size(int hash_type)
 {
 	return hash_type == 2 ? 32 : hash_type == 3 ? 48 : hash_type == 4 ? 64 : hash_type == 5 ? 28 : hash_type == 6 ? 32 :
 	       hash_type == 7 ? 48 : hash_type == 8 ? 64 : 0;
 }
 
+/* Any of the seven hashes over a byte source of len bytes; digest: sha2_digest_size(hash_type) bytes.  hash_type must
+ * be one of 2..8. */
+template <class Src> SHA2_D void hash_src(int hash_type, const Src &m, uint64_t len, uint8_t *digest)
+{
+	if (hash_type == 2) sha256_src(m, len, digest);
+	else if (hash_type == 3) sha512_family_src(m, len, digest, kSha384H, 48);
+	else if (hash_type == 4) sha512_family_src(m, len, digest, kSha512H, 64);
+	else sha3_src(m, len, digest, sha2_digest_size(hash_type));
+}
+
+/* H(pre[0 .. npre) || msg[0 .. nmsg)): the prefix lives with the thread, the message in (global) memory */
+SHA2_D void hash_segments(int hash_type, const uint8_t *pre, uint32_t npre, const uint8_t *msg, uint64_t nmsg,
+			  uint8_t *digest)
+{
+	hash_src(hash_type, Seg2{ pre, npre, msg }, (uint64_t)npre + nmsg, digest);
+}
+
+#if defined(__CUDACC__)
 /* messages are concatenated in `msgs`; message i is msgs[off[i] .. off[i+1]); digests are [n][digest_size] */
-__global__ void __launch_bounds__(128) k_sha2_batch(uint32_t n, int hash_type, const uint8_t *__restrict__ msgs,
-						    const uint64_t *__restrict__ off, uint8_t *__restrict__ digests)
+static __global__ void __launch_bounds__(128) k_sha2_batch(uint32_t n, int hash_type, const uint8_t *__restrict__ msgs,
+							   const uint64_t *__restrict__ off, uint8_t *__restrict__ digests)
 {
 	uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= n) return;
@@ -144,5 +201,6 @@ __global__ void __launch_bounds__(128) k_sha2_batch(uint32_t n, int hash_type, c
 	else if (hash_type == 4) sha512_family_device(m, len, out, kSha512H, 64);
 	else sha3_device(m, len, out, ds);
 }
+#endif
 
 } // namespace eccb200

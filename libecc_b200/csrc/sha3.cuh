@@ -18,6 +18,18 @@ namespace eccb200 {
 
 #include "sha3_constants.inc"
 
+/* Byte sources of the hash functions (sha2.cuh as well): m[i] for i < the length the caller passes. */
+struct ByteSpan { /* one contiguous message */
+	const uint8_t *p;
+	SHA3_HD uint32_t operator[](uint64_t i) const { return p[i]; }
+};
+struct Seg2 { /* pre[0 .. npre) followed by msg */
+	const uint8_t *pre;
+	uint32_t npre;
+	const uint8_t *msg;
+	SHA3_HD uint32_t operator[](uint64_t i) const { return i < npre ? pre[i] : msg[i - npre]; }
+};
+
 static SHA3_HD uint64_t rotl64_(uint64_t x, int n) { return n ? ((x << n) | (x >> (64 - n))) : x; }
 
 /* Keccak-f[1600] on 25 lanes, lane (x, y) at index x + 5*y */
@@ -56,7 +68,7 @@ static SHA3_HD void keccak_f1600(uint64_t a[25])
 }
 
 /* digest_bytes in {28, 32, 48, 64} */
-static SHA3_HD void sha3_device(const uint8_t *m, uint64_t len, uint8_t *digest, int digest_bytes)
+template <class Src> SHA3_HD void sha3_src(const Src &m, uint64_t len, uint8_t *digest, int digest_bytes)
 {
 	const int rate = 200 - 2 * digest_bytes;
 	const uint64_t total = ((len + 1 + (uint64_t)rate - 1) / (uint64_t)rate) * (uint64_t)rate; /* padded length */
@@ -85,6 +97,11 @@ static SHA3_HD void sha3_device(const uint8_t *m, uint64_t len, uint8_t *digest,
 		keccak_f1600(st);
 	}
 	for (int i = 0; i < digest_bytes; i++) digest[i] = (uint8_t)(st[i >> 3] >> (8 * (i & 7)));
+}
+
+static SHA3_HD void sha3_device(const uint8_t *m, uint64_t len, uint8_t *digest, int digest_bytes)
+{
+	sha3_src(ByteSpan{ m }, len, digest, digest_bytes);
 }
 
 } // namespace eccb200
