@@ -175,9 +175,14 @@ def test_gpu_double_smul_against_oracle(curve):
     pts, _ = oracle_smul(curve, random_scalars(curve, n, tag=9301))
     ab[0, :qlen] = 0; ab[1, qlen:] = 0; ab[2] = 0                       # a = 0, b = 0, both
     ab[3, :qlen] = ab[3, qlen:]; pts[3] = oracle_smul(curve, np.frombuffer((q - 1).to_bytes(qlen, "big"), np.uint8).reshape(1, qlen))[0][0]
+    a4 = int.from_bytes(ab[4, :qlen].tobytes(), "big") % q or 1         # a*G == b*(5G): the final addition doubles
+    ab[4] = np.frombuffer(a4.to_bytes(qlen, "big") + (a4 * pow(5, -1, q) % q).to_bytes(qlen, "big"), np.uint8)
+    pts[4] = oracle_smul(curve, np.frombuffer((5).to_bytes(qlen, "big"), np.uint8).reshape(1, qlen))[0][0]
     pts[5, plen - 1] ^= 1                                               # key off the curve
     want, wst = oracle_double_smul(curve, ab, pts)
     assert wst[2] == 1 and wst[3] == 1 and wst[5] == -1                 # aG + a(q-1)G = infinity
+    assert wst[4] == 0 and (want[4] == oracle_smul(curve, np.frombuffer((2 * a4 % q).to_bytes(qlen, "big"),
+                                                                        np.uint8).reshape(1, qlen))[0][0]).all()
     eng = libecc_b200.Engine(curve, comb_window=9)
     got, gst = eng.double_smul_batch(ab, pts)
     eng.close()
