@@ -264,6 +264,54 @@ int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash
 					const uint8_t *d_randomness, const uint8_t *d_msgs,
 					const uint64_t *d_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream);
 
+/*
+ * Batched ECKCDSA / ECGDSA / ECRDSA / SM2 signing of raw messages, hashed on the device: k*G (comb), batched
+ * normalisation, then one kernel that hashes and computes r and s per item.  W = k*G affine, x the private scalar, k
+ * the caller's nonce (what the reference's `rand` callback would return), each scheme as the reference's default build:
+ *   ECCB200_ALG_ECKCDSA h = H(z || m), z the first block-size bytes of Y_x || Y_y (zero-padded or cut);
+ *                       r = H(W_x); both keep their rightmost r_len = min(hsize, qlen) bytes; e = OS2I(r XOR h) mod q;
+ *                       s = x*(k - e) mod q;  sig r || s, r_len + qlen bytes    (src/sig/eckcdsa.c:202-471)
+ *   ECCB200_ALG_ECGDSA  e = -(leftmost bitlen(q) bits of H(m)) mod q, r = W_x mod q, s = x*(k*r + e) mod q;
+ *                       sig r || s, 2*qlen bytes                                 (src/sig/ecgdsa.c:181-347)
+ *   ECCB200_ALG_ECRDSA  e = OS2I(byte-reversed H(m)) mod q, 0 replaced by 1, r = W_x mod q, s = r*x + k*e mod q;
+ *                       sig r || s, 2*qlen bytes                                 (src/sig/ecrdsa.c:196-346)
+ *   ECCB200_ALG_SM2     Z = H(ENTL || ID || a || b || G_x || G_y || Y_x || Y_y), e = OS2I(H(Z || m)),
+ *                       r = (e + W_x) mod q, s = (1 + x)^-1 * (k - r*x) mod q;  sig r || s, 2*qlen bytes
+ *                       (src/sig/sm2.c:136-455; like the reference, no restart on r + k == q)
+ *   privkeys   : n * qlen bytes, x in [1, q-1], for SM2 in [1, q-2] (else ECCB200_ERR)
+ *   pubkeys    : n * 2*plen affine, ECKCDSA and SM2 only (ignored otherwise): Y enters z / Z as given, without a check
+ *                against x; off the curve: ECCB200_ERR
+ *   nonces     : n * qlen bytes, k in [1, q-1] (else ECCB200_ERR)
+ *   msgs / offsets : message i is msgs[offsets[i] .. offsets[i+1]), offsets has n + 1 entries, starts at 0 and never
+ *                decreases (checked here; the _dev form does not re-check it)
+ *   ids / id_offsets : SM2 only (ignored otherwise), the same layout: item i's ID is ids[id_offsets[i] ..
+ *                id_offsets[i+1]), at most 8191 bytes (SM2_MAX_ID_LEN; checked here, an ECCB200_ERR item in the _dev
+ *                form); an empty ID is valid
+ *   hash_type  : 2 .. 8 (SHA256, SHA384, SHA512, SHA3_224 .. SHA3_512) or 11 (SM3); only these two entry points take SM3
+ *   sigs       : [n][eccb200_sign_sig_len], zero unless status is OK
+ *   status     : ECCB200_OK / ECCB200_ERR / ECCB200_RETRY (the reference would restart and a fresh nonce would succeed:
+ *                r == 0 for ECGDSA / ECRDSA / SM2, s == 0 for all four)
+ * Any other sig_type (the Schnorr family and ECDSA have their own entry points), any other hash_type, or SM2 without
+ * ids, or ECKCDSA / SM2 without pubkeys, returns -1 (eccb200_last_error) and writes nothing.  The _dev form follows the
+ * rules of every *_dev entry point (one scratch set per context, calls chained across streams; 16-byte alignment of
+ * the privkey, pubkey, nonce and signature buffers on the 256/384/512-bit curves, not of d_msgs or d_ids).
+ * NOTE: like every entry point of this library this is a throughput path, NOT a constant-time one.
+ */
+#define ECCB200_ALG_ECKCDSA 2
+#define ECCB200_ALG_ECGDSA 6
+#define ECCB200_ALG_ECRDSA 7
+#define ECCB200_ALG_SM2 8
+#define ECCB200_HASH_SM3 11
+int eccb200_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *privkeys,
+			    const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *offsets,
+			    const uint8_t *ids, const uint64_t *id_offsets, uint8_t *sigs, int8_t *status);
+int eccb200_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *d_privkeys,
+				const uint8_t *d_pubkeys, const uint8_t *d_nonces, const uint8_t *d_msgs,
+				const uint64_t *d_offsets, const uint8_t *d_ids, const uint64_t *d_id_offsets,
+				uint8_t *d_sigs, int8_t *d_status, void *stream);
+/* Signature length in bytes of eccb200_sign_msgs_batch on this context's curve, or -1 (unsupported sig_type / hash). */
+int eccb200_sign_sig_len(eccb200_ctx *ctx, int sig_type, int hash_type);
+
 /* cudaMemcpy device -> host (for callers that do not link the CUDA runtime). */
 int eccb200_copy_to_host(eccb200_ctx *ctx, void *host_dst, const void *d_src, size_t bytes);
 

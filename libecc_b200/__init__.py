@@ -41,7 +41,8 @@ ABI_SYMBOLS = [
     "eccb200_fp_addsub_batch", "eccb200_ecdsa_verify_prj_batch", "eccb200_bip0340_verify_batch",
     "eccb200_bip0340_verify_batch_dev", "eccb200_push_results", "eccb200_bind_thread_near_device",
     "eccb200_pipeline_chunk_bounds", "eccb200_double_smul_batch", "eccb200_double_smul_batch_dev",
-    "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev",
+    "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev", "eccb200_sign_msgs_batch",
+    "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len",
 ]
 
 _lib = None
@@ -122,6 +123,11 @@ def load_library() -> ctypes.CDLL:
                                                     i8p]
     lib.eccb200_schnorr_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp,
                                                         u8p, i8p, vp]
+    lib.eccb200_sign_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp, u8p, vp, u8p,
+                                            i8p]
+    lib.eccb200_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp, u8p, vp,
+                                                u8p, i8p, vp]
+    lib.eccb200_sign_sig_len.argtypes = [vp, ctypes.c_int, ctypes.c_int]
     lib.eccb200_copy_to_host.argtypes = [vp, vp, vp, ctypes.c_size_t]
     lib.eccb200_bind_thread_near_device.argtypes = [ctypes.c_int]
     lib.eccb200_pipeline_chunk_bounds.argtypes = [u32, u32, u32, u32, ctypes.c_int, vp, ctypes.c_int]
@@ -381,6 +387,46 @@ class Engine:
             d_pubkeys.data_ptr() if d_pubkeys is not None else None, d_randomness.data_ptr(), d_msgs.data_ptr(),
             d_offsets.data_ptr(), d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)),
             "eccb200_schnorr_sign_msgs_batch_dev")
+
+    SIGN_ALGS = {"ECKCDSA": 2, "ECGDSA": 6, "ECRDSA": 7, "SM2": 8}  # libecc ec_alg_type values
+    SIGN_HASH_IDS = dict(HASH_IDS, SM3=11)  # the message signers also hash with SM3
+
+    def sign_sig_len(self, alg: str, hash_name: str) -> int:
+        n = self.lib.eccb200_sign_sig_len(self._h, self.SIGN_ALGS[alg], self.SIGN_HASH_IDS[hash_name])
+        self._check(0 if n > 0 else -1, "eccb200_sign_sig_len")
+        return n
+
+    def sign_msgs_batch(self, alg: str, hash_name: str, privkeys, nonces, msgs, pubkeys=None,
+                        ids=None) -> Tuple[np.ndarray, np.ndarray]:
+        """ECKCDSA / ECGDSA / ECRDSA / SM2 signatures of raw messages, hashed on the device (hash_name may be "SM3").
+        nonces[i] is the k the reference's rand callback would return (qlen bytes).  pubkeys (n*2*plen affine) are
+        required for ECKCDSA and SM2, ids (a list of byte strings, the SM2 user IDs) for SM2.  Returns
+        (sigs[n, siglen], status[n]): 0 OK, -1 ERR, 2 RETRY (see include/libecc_b200.h)."""
+        n = len(msgs)
+        d = _as_u8(privkeys, n * self.qlen)
+        k = _as_u8(nonces, n * self.qlen)
+        pk = _as_u8(pubkeys, n * 2 * self.plen) if pubkeys is not None else None
+        blob, off = self._pack_msgs(msgs)
+        id_blob, id_off = self._pack_msgs(ids) if ids is not None else (None, None)
+        sigs = np.zeros((n, self.sign_sig_len(alg, hash_name)), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_sign_msgs_batch(
+            self._h, self.SIGN_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, d.ctypes.data,
+            pk.ctypes.data if pk is not None else None, k.ctypes.data, blob.ctypes.data, off.ctypes.data,
+            id_blob.ctypes.data if id_blob is not None else None, id_off.ctypes.data if id_off is not None else None,
+            sigs.ctypes.data, status.ctypes.data), "eccb200_sign_msgs_batch")
+        return sigs, status
+
+    def sign_msgs_batch_dev(self, alg: str, hash_name: str, d_privkeys, d_nonces, d_msgs, d_offsets, d_sigs, d_status,
+                            d_pubkeys=None, d_ids=None, d_id_offsets=None, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`); d_offsets / d_id_offsets: n + 1 uint64 entries, not
+        re-checked."""
+        n = d_privkeys.numel() // self.qlen
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self._check(self.lib.eccb200_sign_msgs_batch_dev(
+            self._h, self.SIGN_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, d_privkeys.data_ptr(), ptr(d_pubkeys),
+            d_nonces.data_ptr(), d_msgs.data_ptr(), d_offsets.data_ptr(), ptr(d_ids), ptr(d_id_offsets),
+            d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_sign_msgs_batch_dev")
 
     def copy_to_host(self, d_ptr: int, nbytes: int) -> np.ndarray:
         out = np.empty(nbytes, dtype=np.uint8)

@@ -22,6 +22,7 @@
 #pragma once
 #include "fp.cuh"
 #include "sha2.cuh"
+#include "sm3.cuh"
 
 namespace eccb200 {
 
@@ -998,6 +999,175 @@ ECC_D int schnorr_sign_core(uint8_t *sig, int sig_type, int hash_type, const uin
 		for (int i = 0; i < rlen; i++) sig[i] = h[i];
 	else
 		for (int i = 0; i < rlen; i++) sig[i] = W[i];
+	store_be<N>(sig + rlen, s, QL);
+	return 0;
+}
+
+/* ------------------------------------------------------------------ message signers (ECKCDSA, ECGDSA, ECRDSA, SM2) */
+
+/* ec_alg_type values of the reference (lib_ecc_types.h) for the randomized signers that hash the raw message */
+enum { SIG_ECKCDSA = 2, SIG_ECGDSA = 6, SIG_ECRDSA = 7, SIG_SM2 = 8 };
+constexpr uint32_t kSm2MaxIdLen = 8191; /* SM2_MAX_ID_LEN: ENTL = 8 * len(ID) fits 16 bits (sig/sm2.c:154) */
+constexpr int kMsgsMaxPrefix = 144;    /* ECKCDSA's z: the largest block size (SHA3-224) */
+
+#if defined(__CUDACC__)
+#define ECC_D_NOINLINE __device__ __noinline__
+#else
+#define ECC_D_NOINLINE __attribute__((noinline))
+#endif
+
+/* r || s: r_len + qlen with r_len = min(hsize, qlen) for ECKCDSA (ECKCDSA_SIGLEN), 2*qlen for the other three */
+template <class C> ECC_HD int msgs_sig_len(int sig_type, int digest_size)
+{
+	return sig_type == SIG_ECKCDSA ? (digest_size < C::QLEN ? digest_size : C::QLEN) + C::QLEN : 2 * C::QLEN;
+}
+
+/* One out-of-line copy of the eight hashes per kernel: the signers hash at up to three places per item. */
+static ECC_D_NOINLINE void msg_hash_seg3(int hash_type, const Seg3 &src, uint64_t len, uint8_t *digest)
+{
+	msg_hash_src(hash_type, src, len, digest);
+}
+
+/* x in [1, q-2] (SM2 keys, sm2_init_pub_key, sig/sm2.c:72-75) or [1, q-1] (the other three) */
+template <class C> ECC_HD bool msgs_key_in_range(int sig_type, const Fe<C::N> &x)
+{
+	typedef Field<typename C::Fq> Fq;
+	if (Fq::is_zero(x) || Fq::geq_mod(x)) return false;
+	if (sig_type != SIG_SM2) return true;
+	Fe<C::N> one, t;
+	Fq::set_zero(one);
+	one.w[0] = 1;
+	Fq::add(t, x, one);
+	return !Fq::is_zero(t);
+}
+
+/* (1 + x) in the Montgomery domain of q: the factor SM2 inverts (step 8, sig/sm2.c:437-441) */
+template <class C> ECC_HD void sm2_one_plus_x(Fe<C::N> &r, const Fe<C::N> &x)
+{
+	typedef Field<typename C::Fq> Fq;
+	Fe<C::N> one, t;
+	Fq::set_zero(one);
+	one.w[0] = 1;
+	Fq::add(t, x, one);
+	Fq::to_mont(r, t);
+}
+
+/* SM2's Z = H(ENTL || ID || a || b || G_x || G_y || Y_x || Y_y) (sm2_compute_Z, sig/sm2.c:136-215): ENTL is held by
+ * the thread, the ID is read where it lies, a || b || G || Y is assembled by the thread; Y is the affine wire key. */
+template <class C> ECC_D void sm2_z(int hash_type, const uint8_t *id, uint32_t idlen, const uint8_t *Y, uint8_t *Z)
+{
+	typedef Field<typename C::Fp> Fp;
+	constexpr int N = C::N, PL = C::PLEN;
+	const uint32_t entl = (idlen * 8u) & 0xffffu;
+	const uint8_t ent[2] = { (uint8_t)(entl >> 8), (uint8_t)entl };
+	uint8_t tail[6 * PL];
+	Fe<N> v, m;
+#pragma unroll
+	for (int i = 0; i < N; i++) m.w[i] = C::A_MONT(i);
+	Fp::from_mont(v, m);
+	store_be<N>(tail, v, PL);
+#pragma unroll
+	for (int i = 0; i < N; i++) m.w[i] = C::B_MONT(i);
+	Fp::from_mont(v, m);
+	store_be<N>(tail + PL, v, PL);
+#pragma unroll
+	for (int i = 0; i < N; i++) v.w[i] = C::GX(i);
+	store_be<N>(tail + 2 * PL, v, PL);
+#pragma unroll
+	for (int i = 0; i < N; i++) v.w[i] = C::GY(i);
+	store_be<N>(tail + 3 * PL, v, PL);
+	for (int i = 0; i < 2 * PL; i++) tail[4 * PL + i] = Y[i];
+	msg_hash_seg3(hash_type, Seg3{ ent, 2, id, idlen, tail }, 2 + (uint64_t)idlen + 6 * PL, Z);
+}
+
+/*
+ * One ECKCDSA / ECGDSA / ECRDSA / SM2 signature from W = k*G (affine wire bytes, as K4 writes them), the private scalar
+ * x and the nonce k (plain integers) and the message (in memory, read where it lies).  Every scheme follows the
+ * reference's default build (sig/eckcdsa.c:202-471, ecgdsa.c:181-347, ecrdsa.c:196-346, sm2.c:136-455):
+ *   ECGDSA  e = -(leftmost bitlen(q) bits of H(m)) mod q, r = W_x mod q, s = x*(k*r + e) mod q
+ *   ECRDSA  e = OS2I(byte-reversed H(m)) mod q (0 -> 1), r = W_x mod q, s = r*x + k*e mod q
+ *   ECKCDSA r = the rightmost r_len = min(hsize, qlen) bytes of H(W_x), h those of H(z || m) with z the first
+ *           block-size bytes of Y_x || Y_y || 0...; e = OS2I(r XOR h) mod q, s = x*(k - e) mod q
+ *   SM2     e = OS2I(H(Z || m)) (sm2_z), r = (e + W_x) mod q, s = (1 + x)^-1 * (k - r*x) mod q with inv1x = (1 + x)^-1
+ *           in the Montgomery domain of q (the caller inverts, CTA-wide on the device).  Like the reference (step 7,
+ *           sig/sm2.c:406-411 compares r + q with q) there is no restart on r + k == q.
+ * Y is the affine wire key (ECKCDSA and SM2; key_ok: on the curve), id / idlen SM2's ID.
+ * Returns 0 (sig written), -1 (x outside [1, q-1] (SM2: [1, q-2]), k outside [1, q-1], a key off the curve or an ID
+ * longer than 8191 bytes) or 2 (a reference restart: r == 0 for ECGDSA / ECRDSA / SM2, s == 0 for all four); sig
+ * (msgs_sig_len bytes) is zero unless 0 is returned.
+ */
+template <class C>
+ECC_D int msgs_sign_core(uint8_t *sig, int sig_type, int hash_type, const uint8_t *W, const Fe<C::N> &x,
+			 const Fe<C::N> &k, const uint8_t *msg, uint64_t mlen, const uint8_t *Y, bool key_ok,
+			 const uint8_t *id, uint32_t idlen, const Fe<C::N> &inv1x)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, PL = C::PLEN, QL = C::QLEN;
+	const int ds = msg_hash_digest_size(hash_type);
+	const int siglen = msgs_sig_len<C>(sig_type, ds);
+	const bool sm2 = sig_type == SIG_SM2;
+	if (!key_ok || !msgs_key_in_range<C>(sig_type, x) || Fq::is_zero(k) || Fq::geq_mod(k) || (sm2 && idlen > kSm2MaxIdLen)) {
+		for (int i = 0; i < siglen; i++) sig[i] = 0;
+		return -1;
+	}
+	uint8_t pre[kMsgsMaxPrefix], h[64];
+	Fe<N> e, r, s, t, xm, km;
+	Fq::to_mont(xm, x);
+	Fq::to_mont(km, k);
+	load_be<N>(r, W, PL);
+	scalar_reduce<C>(r); /* W_x mod q */
+	bool retry = false;
+	int rlen = QL, shift = 0;
+	if (sig_type == SIG_ECKCDSA) {
+		const int bs = msg_hash_block_size(hash_type);
+		for (int i = 0; i < bs; i++) pre[i] = i < 2 * PL ? Y[i] : 0u;
+		uint8_t hr[64];
+		msg_hash_seg3(hash_type, Seg3{ pre, (uint32_t)bs, msg, mlen, nullptr }, (uint64_t)bs + mlen, h); /* H(z || m) */
+		msg_hash_seg3(hash_type, Seg3{ W, (uint32_t)PL, nullptr, 0, nullptr }, (uint64_t)PL, hr);      /* H(W_x)    */
+		rlen = ds < QL ? ds : QL;
+		shift = ds - rlen;
+		for (int i = 0; i < rlen; i++) {
+			h[i] = h[shift + i] ^ hr[shift + i];
+			pre[i] = hr[shift + i];
+		}
+		digest_full_mod_q<C>(e, h, (uint32_t)rlen);
+		Fq::sub(t, k, e);
+		Fq::mul(s, t, xm); /* x*(k - e) */
+	} else if (sm2) {
+		sm2_z<C>(hash_type, id, idlen, Y, pre);
+		msg_hash_seg3(hash_type, Seg3{ pre, (uint32_t)ds, msg, mlen, nullptr }, (uint64_t)ds + mlen, h);
+		digest_full_mod_q<C>(e, h, (uint32_t)ds);
+		Fq::add(r, e, r);  /* (OS2I(H) + W_x) mod q */
+		retry = Fq::is_zero(r);
+		Fq::mul(t, r, xm); /* r*x */
+		Fq::sub(t, k, t);
+		Fq::mul(s, t, inv1x);
+	} else {
+		msg_hash_seg3(hash_type, Seg3{ nullptr, 0, msg, mlen, nullptr }, mlen, h);
+		retry = Fq::is_zero(r);
+		if (sig_type == SIG_ECGDSA) {
+			digest_to_scalar<C>(e, h, (uint32_t)ds);
+			Fq::neg(e, e);
+			Fq::mul(t, r, km); /* k*r */
+			Fq::add(t, t, e);
+			Fq::mul(s, t, xm);
+		} else {
+			for (int i = 0; i < ds; i++) pre[i] = h[ds - 1 - i];
+			digest_full_mod_q<C>(e, pre, (uint32_t)ds);
+			if (Fq::is_zero(e)) e.w[0] = 1;
+			Fq::mul(t, r, xm); /* r*x */
+			Fq::mul(s, e, km); /* k*e */
+			Fq::add(s, s, t);
+		}
+	}
+	if (retry || Fq::is_zero(s)) {
+		for (int i = 0; i < siglen; i++) sig[i] = 0;
+		return 2;
+	}
+	if (sig_type == SIG_ECKCDSA)
+		for (int i = 0; i < rlen; i++) sig[i] = pre[i];
+	else
+		store_be<N>(sig, r, QL);
 	store_be<N>(sig + rlen, s, QL);
 	return 0;
 }

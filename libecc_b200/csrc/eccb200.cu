@@ -1680,9 +1680,109 @@ extern "C" int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_typ
 				d_status, ctx->jac, ctx->prefix, ctx->aff, ctx->sign_k, (cudaStream_t)stream);
 }
 
-/* Host-pointer form: chunks of four waves on two streams like eccb200_ecdsa_verify_msgs_batch (a chunk's copies
- * overlap the other chunk's kernels), K1 / K4 scratch from the per-stream stage buffers, the chunk's message bytes
- * addressed with the caller's absolute offsets against a shifted base. */
+/* A per-item input of the host-pointer message signers: `width` bytes per item (host == nullptr: not used) */
+struct SignCol {
+	const uint8_t *host;
+	size_t width;
+};
+/* A ragged input: item i's bytes are data[off[i] .. off[i+1]) (off == nullptr: not used) */
+struct SignRagged {
+	const uint8_t *data;
+	const uint64_t *off;
+};
+/* One chunk's device buffers, in the order of the inputs (nullptr where an input is not used).  rag_base[j] is shifted
+ * so that the caller's absolute offsets address it: the chunk's bytes start at off[lo]. */
+struct SignChunk {
+	const uint8_t *col[3];
+	uint8_t *scratch; /* scratch_width bytes per item */
+	const uint8_t *rag_base[2];
+	const uint64_t *rag_off[2];
+	uint8_t *sigs;
+	int8_t *status;
+};
+
+/* Host-pointer form of the message signers (Schnorr family and the others): chunks of four waves on two streams like
+ * eccb200_ecdsa_verify_msgs_batch (a chunk's copies overlap the other chunk's kernels), K1 / K4 scratch from the
+ * per-stream stage buffers.  launch(s, cnt, chunk) queues one chunk's kernels on ctx->streams[s].  The caller has
+ * checked the offsets. */
+template <class Launch>
+static int sign_msgs_pipeline(eccb200_ctx *ctx, uint32_t n, const SignCol (&cols)[3], size_t scratch_width,
+			      const SignRagged (&rag)[2], size_t siglen, uint8_t *sigs, int8_t *status, Launch launch)
+{
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_stages(ctx, 1, 1)) return -1; /* the stage_jac / stage_prefix / stage_aff scratch */
+	const uint32_t step = std::min(ctx->chunk_eq, ctx->chunk);
+	size_t max_rag[2] = { 0, 0 };
+	for (uint32_t lo = 0; lo < n; lo += step) {
+		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n);
+		for (int j = 0; j < 2; j++)
+			if (rag[j].off) max_rag[j] = std::max<size_t>(max_rag[j], (size_t)(rag[j].off[hi] - rag[j].off[lo]));
+	}
+	const uint32_t cap = std::min(step, n);
+	size_t b_col[3], b_rag[2], b_roff[2];
+	size_t stage = 0;
+	for (int j = 0; j < 3; j++) stage += b_col[j] = cols[j].host ? align16(cap * cols[j].width) : 0;
+	const size_t b_k = align16(cap * scratch_width);
+	for (int j = 0; j < 2; j++) {
+		stage += b_rag[j] = rag[j].off ? align16(max_rag[j] + 16) : 0;
+		stage += b_roff[j] = rag[j].off ? align16(((size_t)cap + 1) * sizeof(uint64_t)) : 0;
+	}
+	const size_t b_sig = align16(cap * siglen), b_st = align16(cap);
+	stage += b_k + b_sig + b_st;
+	uint8_t *d = nullptr;
+	CUDA_OK(cudaMalloc(&d, 2 * stage));
+	int rc = 0;
+	uint32_t c = 0;
+	for (uint32_t lo = 0; lo < n && !rc; lo += step, c++) {
+		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n), cnt = hi - lo;
+		const int s = (int)(c & 1);
+		cudaStream_t st = ctx->streams[s];
+		uint8_t *p = d + (size_t)s * stage;
+		SignChunk ch = {};
+		bool ok = true;
+		for (int j = 0; j < 3; j++) {
+			if (cols[j].host) {
+				ok = ok && cudaMemcpyAsync(p, cols[j].host + lo * cols[j].width, cnt * cols[j].width,
+							   cudaMemcpyHostToDevice, st) == cudaSuccess;
+				ch.col[j] = p;
+			}
+			p += b_col[j];
+		}
+		ch.scratch = scratch_width ? p : nullptr;
+		p += b_k;
+		for (int j = 0; j < 2; j++) {
+			if (rag[j].off) {
+				const uint64_t *off = rag[j].off;
+				const size_t bytes = (size_t)(off[hi] - off[lo]);
+				ok = ok && (!bytes || cudaMemcpyAsync(p, rag[j].data + off[lo], bytes, cudaMemcpyHostToDevice, st) ==
+							      cudaSuccess);
+				ok = ok && cudaMemcpyAsync(p + b_rag[j], off + lo, ((size_t)cnt + 1) * sizeof(uint64_t),
+							   cudaMemcpyHostToDevice, st) == cudaSuccess;
+				ch.rag_base[j] = p - off[lo]; /* the kernels add the caller's absolute offsets to this base */
+				ch.rag_off[j] = (const uint64_t *)(p + b_rag[j]);
+			}
+			p += b_rag[j] + b_roff[j];
+		}
+		ch.sigs = p;
+		ch.status = (int8_t *)(p + b_sig);
+		if (!ok) {
+			rc = fail("H2D copy failed");
+			break;
+		}
+		rc = launch(s, cnt, ch);
+		if (!rc && (cudaMemcpyAsync(sigs + lo * siglen, ch.sigs, cnt * siglen, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+			    cudaMemcpyAsync(status + lo, ch.status, cnt, cudaMemcpyDeviceToHost, st) != cudaSuccess))
+			rc = fail("D2H copy failed");
+	}
+	const std::string keep = g_err;
+	for (int s2 = 0; s2 < 2; s2++)
+		if (cudaStreamSynchronize(ctx->streams[s2]) != cudaSuccess && !rc) rc = fail("stream synchronisation failed");
+	if (rc && !keep.empty()) g_err = keep;
+	cudaFree(d);
+	return rc;
+}
+
+/* Host-pointer form through sign_msgs_pipeline; the BIP0340 nonces go to the chunk's scratch column. */
 extern "C" int eccb200_schnorr_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
 					       const uint8_t *privkeys, const uint8_t *pubkeys, const uint8_t *randomness,
 					       const uint8_t *msgs, const uint64_t *offsets, uint8_t *sigs, int8_t *status)
@@ -1696,59 +1796,132 @@ extern "C" int eccb200_schnorr_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, i
 	if (n == 0) return 0;
 	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
 	if (offsets[n] && !msgs) return fail("null argument");
-	CUDA_OK(cudaSetDevice(ctx->device));
-	if (ensure_stages(ctx, 1, 1)) return -1; /* the stage_jac / stage_prefix / stage_aff scratch */
-	const uint32_t step = std::min(ctx->chunk_eq, ctx->chunk);
-	const size_t ql = ctx->qlen, pki = bip ? 2 * (size_t)ctx->plen : 0;
+	const size_t ql = ctx->qlen;
 	size_t siglen = 0;
 	dispatch(ctx->curve_id, [&](auto c) {
 		siglen = (size_t)schnorr_sig_len<decltype(c)>(sig_type, ds);
 		return 0;
 	});
-	size_t max_msg = 0;
-	for (uint32_t lo = 0; lo < n; lo += step) {
-		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n);
-		max_msg = std::max<size_t>(max_msg, (size_t)(offsets[hi] - offsets[lo]));
+	const SignCol cols[3] = { { privkeys, ql }, { bip ? pubkeys : nullptr, 2 * (size_t)ctx->plen }, { randomness, ql } };
+	const SignRagged rag[2] = { { msgs, offsets }, { nullptr, nullptr } };
+	return sign_msgs_pipeline(ctx, n, cols, bip ? ql : 0, rag, siglen, sigs, status,
+				  [&](int s, uint32_t cnt, const SignChunk &ch) {
+					  return schnorr_sign_dev(ctx, sig_type, hash_type, cnt, ch.col[0], ch.col[1],
+								  ch.col[2], ch.rag_base[0], ch.rag_off[0], ch.sigs,
+								  ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
+								  ctx->stage_aff[s], ch.scratch, ctx->streams[s]);
+				  });
+}
+
+/* ------------------------------------------------------------------------- ECKCDSA / ECGDSA / ECRDSA / SM2 sign */
+
+static const char *kMsgsAlgMsg = "unsupported sig_type (ECKCDSA = 2, ECGDSA = 6, ECRDSA = 7, SM2 = 8)";
+static const char *kMsgsHashMsg = "unsupported hash (SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224..512 = 5..8, SM3 = 11)";
+static bool msgs_alg_ok(int sig_type)
+{
+	return sig_type == SIG_ECKCDSA || sig_type == SIG_ECGDSA || sig_type == SIG_ECRDSA || sig_type == SIG_SM2;
+}
+
+/* the checks both forms share; 0, or -1 with the reason in eccb200_last_error */
+static int msgs_sign_args(const eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const void *privkeys,
+			  const void *pubkeys, const void *nonces, const void *offsets, const void *ids,
+			  const void *id_offsets, const void *sigs, const void *status)
+{
+	if (!ctx) return fail("null argument");
+	if (!msgs_alg_ok(sig_type)) return fail(kMsgsAlgMsg);
+	if (!msg_hash_digest_size(hash_type)) return fail(kMsgsHashMsg);
+	const bool sm2 = sig_type == SIG_SM2;
+	if (n && (!privkeys || !nonces || !offsets || !sigs || !status || ((sm2 || sig_type == SIG_ECKCDSA) && !pubkeys) ||
+		  (sm2 && (!ids || !id_offsets))))
+		return fail("null argument");
+	return 0;
+}
+
+static size_t msgs_siglen(const eccb200_ctx *ctx, int sig_type, int hash_type)
+{
+	size_t siglen = 0;
+	dispatch(ctx->curve_id, [&](auto c) {
+		siglen = (size_t)msgs_sig_len<decltype(c)>(sig_type, msg_hash_digest_size(hash_type));
+		return 0;
+	});
+	return siglen;
+}
+
+extern "C" int eccb200_sign_sig_len(eccb200_ctx *ctx, int sig_type, int hash_type)
+{
+	if (!ctx) return fail("null argument");
+	if (!msgs_alg_ok(sig_type)) return fail(kMsgsAlgMsg);
+	if (!msg_hash_digest_size(hash_type)) return fail(kMsgsHashMsg);
+	return (int)msgs_siglen(ctx, sig_type, hash_type);
+}
+
+/* K1 on the nonces, K4, finish kernel — all on `st`.  SM2's finish runs on the normalisation's grid (several items per
+ * thread share the CTA-wide inversion of 1 + x); the other schemes invert nothing and run one item per thread. */
+static int msgs_sign_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *d_priv,
+			 const uint8_t *d_pub, const uint8_t *d_nonce, const uint8_t *d_msgs, const uint64_t *d_off,
+			 const uint8_t *d_ids, const uint64_t *d_id_off, uint8_t *d_sigs, int8_t *d_status, uint32_t *jac,
+			 uint32_t *prefix, uint8_t *aff, cudaStream_t st)
+{
+	if (n == 0) return 0;
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		LaunchFixed<C>::fixed(n, d_nonce, ctx->table, ctx->w, jac, d_status, st);       /* W = k*G  */
+		LaunchMisc<C>::to_affine(affine_grid(ctx, n), n, jac, prefix, aff, d_status, st); /* affine W */
+		LaunchMisc<C>::msgs_sign_finish(sig_type == SIG_SM2 ? affine_grid(ctx, n) : grid_for(n), n, sig_type,
+						hash_type, d_priv, d_pub, d_nonce, d_msgs, d_off, d_ids, d_id_off, aff,
+						prefix, d_sigs, d_status, st);                 /* hash, r, s */
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 3;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+extern "C" int eccb200_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					   const uint8_t *d_privkeys, const uint8_t *d_pubkeys, const uint8_t *d_nonces,
+					   const uint8_t *d_msgs, const uint64_t *d_offsets, const uint8_t *d_ids,
+					   const uint64_t *d_id_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream)
+{
+	if (msgs_sign_args(ctx, sig_type, hash_type, n, d_privkeys, d_pubkeys, d_nonces, d_offsets, d_ids, d_id_offsets,
+			   d_sigs, d_status))
+		return -1;
+	if (misaligned16(ctx, { d_privkeys, d_pubkeys, d_nonces, d_sigs })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_work(ctx, n)) return -1;
+	const bool sm2 = sig_type == SIG_SM2, with_key = sm2 || sig_type == SIG_ECKCDSA;
+	return msgs_sign_dev(ctx, sig_type, hash_type, n, d_privkeys, with_key ? d_pubkeys : nullptr, d_nonces, d_msgs,
+			     d_offsets, sm2 ? d_ids : nullptr, sm2 ? d_id_offsets : nullptr, d_sigs, d_status, ctx->jac,
+			     ctx->prefix, ctx->aff, (cudaStream_t)stream);
+}
+
+extern "C" int eccb200_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+				       const uint8_t *privkeys, const uint8_t *pubkeys, const uint8_t *nonces,
+				       const uint8_t *msgs, const uint64_t *offsets, const uint8_t *ids,
+				       const uint64_t *id_offsets, uint8_t *sigs, int8_t *status)
+{
+	if (msgs_sign_args(ctx, sig_type, hash_type, n, privkeys, pubkeys, nonces, offsets, ids, id_offsets, sigs, status))
+		return -1;
+	if (n == 0) return 0;
+	const bool sm2 = sig_type == SIG_SM2, with_key = sm2 || sig_type == SIG_ECKCDSA;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	if (sm2) {
+		if (!offsets_ok(id_offsets, n)) return fail("id_offsets must start at 0 and be non-decreasing");
+		for (uint32_t i = 0; i < n; i++)
+			if (id_offsets[i + 1] - id_offsets[i] > kSm2MaxIdLen) return fail("SM2 ID longer than 8191 bytes");
 	}
-	const uint32_t cap = std::min(step, n);
-	const size_t b_x = align16(cap * ql), b_pk = align16(cap * pki), b_r = align16(cap * ql),
-		     b_k = bip ? align16(cap * ql) : 0, b_msg = align16(max_msg + 16),
-		     b_off = align16(((size_t)cap + 1) * sizeof(uint64_t)), b_sig = align16(cap * siglen), b_st = align16(cap);
-	const size_t stage = b_x + b_pk + b_r + b_k + b_msg + b_off + b_sig + b_st;
-	uint8_t *d = nullptr;
-	CUDA_OK(cudaMalloc(&d, 2 * stage));
-	int rc = 0;
-	uint32_t c = 0;
-	for (uint32_t lo = 0; lo < n && !rc; lo += step, c++) {
-		const uint32_t hi = (uint32_t)std::min<uint64_t>((uint64_t)lo + step, n), cnt = hi - lo;
-		const int s = (int)(c & 1);
-		cudaStream_t st = ctx->streams[s];
-		uint8_t *d_x = d + (size_t)s * stage, *d_pk = d_x + b_x, *d_r = d_pk + b_pk, *d_k = d_r + b_r, *d_msg = d_k + b_k,
-			*d_off = d_msg + b_msg, *d_sig = d_off + b_off, *d_st = d_sig + b_sig;
-		const size_t mbytes = (size_t)(offsets[hi] - offsets[lo]);
-		if (cudaMemcpyAsync(d_x, privkeys + lo * ql, cnt * ql, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-		    (bip && cudaMemcpyAsync(d_pk, pubkeys + lo * pki, cnt * pki, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
-		    cudaMemcpyAsync(d_r, randomness + lo * ql, cnt * ql, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-		    (mbytes && cudaMemcpyAsync(d_msg, msgs + offsets[lo], mbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) ||
-		    cudaMemcpyAsync(d_off, offsets + lo, ((size_t)cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st) !=
-			    cudaSuccess) {
-			rc = fail("H2D copy failed");
-			break;
-		}
-		/* the kernels add the caller's absolute offsets to this base: the chunk's bytes start at offsets[lo] */
-		rc = schnorr_sign_dev(ctx, sig_type, hash_type, cnt, d_x, bip ? d_pk : nullptr, d_r, d_msg - offsets[lo],
-				      (const uint64_t *)d_off, d_sig, (int8_t *)d_st, ctx->stage_jac[s], ctx->stage_prefix[s],
-				      ctx->stage_aff[s], d_k, st);
-		if (!rc && (cudaMemcpyAsync(sigs + lo * siglen, d_sig, cnt * siglen, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-			    cudaMemcpyAsync(status + lo, d_st, cnt, cudaMemcpyDeviceToHost, st) != cudaSuccess))
-			rc = fail("D2H copy failed");
-	}
-	const std::string keep = g_err;
-	for (int s2 = 0; s2 < 2; s2++)
-		if (cudaStreamSynchronize(ctx->streams[s2]) != cudaSuccess && !rc) rc = fail("stream synchronisation failed");
-	if (rc && !keep.empty()) g_err = keep;
-	cudaFree(d);
-	return rc;
+	const size_t ql = ctx->qlen;
+	const SignCol cols[3] = { { privkeys, ql }, { with_key ? pubkeys : nullptr, 2 * (size_t)ctx->plen }, { nonces, ql } };
+	const SignRagged rag[2] = { { msgs, offsets }, { sm2 ? ids : nullptr, sm2 ? id_offsets : nullptr } };
+	return sign_msgs_pipeline(ctx, n, cols, 0, rag, msgs_siglen(ctx, sig_type, hash_type), sigs, status,
+				  [&](int s, uint32_t cnt, const SignChunk &ch) {
+					  return msgs_sign_dev(ctx, sig_type, hash_type, cnt, ch.col[0], ch.col[1], ch.col[2],
+							       ch.rag_base[0], ch.rag_off[0], ch.rag_base[1], ch.rag_off[1],
+							       ch.sigs, ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
+							       ctx->stage_aff[s], ctx->streams[s]);
+				  });
 }
 
 /* cudaMemcpy device -> host for callers that do not link the CUDA runtime (bench.py reads peer-written buffers). */

@@ -1069,6 +1069,90 @@ __global__ void __launch_bounds__(128) k_ecdsa_sign_finish(uint32_t n, const uin
 	}
 }
 
+/* ------------------------------------------------------------------------- ECKCDSA / ECGDSA / ECRDSA / SM2 sign */
+
+/*
+ * After K1 (k*G) and K4 (affine W): the hashes over the message (and SM2's Z, ECKCDSA's z and H(W_x)), then r and s
+ * (msgs_sign_core).  Each thread owns items tid, tid + T, ... (T = the grid's threads), like k_ecdsa_sign_finish.  For
+ * SM2, (1 + x)^-1 mod q comes from the same two-level simultaneous inversion: a serial prefix product over the
+ * thread's items (prefix scratch), one CTA-wide inversion, then the items in reverse order.  Items whose x is outside
+ * [1, q-2] stay out of the product.  The other schemes invert nothing and run one item per thread.
+ * Messages / IDs as k_sha2_batch: item i's are msgs[off[i] .. off[i+1]) and ids[id_off[i] .. id_off[i+1]).
+ * sigs: [n][msgs_sig_len], status: 0 / -1 / 2 (ECCB200_OK / _ERR / _RETRY).
+ */
+template <class C>
+__global__ void __launch_bounds__(128) k_msgs_sign_finish(uint32_t n, int sig_type, int hash_type,
+							  const uint8_t *__restrict__ privkeys,
+							  const uint8_t *__restrict__ pubkeys,
+							  const uint8_t *__restrict__ nonces,
+							  const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+							  const uint8_t *__restrict__ ids,
+							  const uint64_t *__restrict__ id_off,
+							  const uint8_t *__restrict__ W_aff, uint32_t *__restrict__ prefix,
+							  uint8_t *__restrict__ sigs, int8_t *__restrict__ status)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N;
+	const bool sm2 = sig_type == SIG_SM2;
+	const uint32_t T = gridDim.x * blockDim.x;
+	const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+	const bool active = tid < n;
+	Fe<N> inv;
+	Fq::set_one(inv);
+	uint32_t last = tid;
+	if (active) last = tid + (n - 1 - tid) / T * T;
+	if (sm2) {
+		Fe<N> acc;
+		Fq::set_one(acc);
+		if (active) {
+			for (uint32_t e = tid; e < n; e += T) {
+				Fe<N> x;
+				load_wire<N, C::QLEN>(x, privkeys + (size_t)e * C::QLEN);
+				store_words<N>(prefix + (size_t)e * N, acc);
+				if (msgs_key_in_range<C>(SIG_SM2, x)) {
+					Fe<N> t, u;
+					sm2_one_plus_x<C>(u, x);
+					Fq::mul(t, acc, u);
+					acc = t;
+				}
+				if (n - e <= T) break;
+			}
+		}
+		__shared__ uint32_t sh_inv[ECC_CTA_INV_WORDS(N)];
+		cta_inverse_128<typename C::Fq>(inv, acc, sh_inv);
+	}
+	if (!active) return;
+	const int siglen = msgs_sig_len<C>(sig_type, msg_hash_digest_size(hash_type));
+	const bool with_key = sm2 || sig_type == SIG_ECKCDSA;
+	for (uint32_t e = last;; e -= T) {
+		Fe<N> x, k, ix;
+		load_wire<N, C::QLEN>(x, privkeys + (size_t)e * C::QLEN);
+		load_wire<N, C::QLEN>(k, nonces + (size_t)e * C::QLEN);
+		Fq::set_zero(ix);
+		if (sm2 && msgs_key_in_range<C>(SIG_SM2, x)) {
+			Fe<N> pre, u, t;
+			load_words<N>(pre, prefix + (size_t)e * N);
+			Fq::mul(ix, inv, pre); /* (1 + x)^-1 in Montgomery form */
+			sm2_one_plus_x<C>(u, x);
+			Fq::mul(t, inv, u);
+			inv = t;
+		}
+		const uint8_t *pk = with_key ? pubkeys + (size_t)e * (2 * C::PLEN) : nullptr;
+		bool key_ok = true;
+		if (with_key) {
+			Aff<C> P;
+			key_ok = load_affine_checked<C>(P, pk);
+		}
+		const uint8_t *id = sm2 ? ids + id_off[e] : nullptr;
+		const uint64_t idlen = sm2 ? id_off[e + 1] - id_off[e] : 0;
+		status[e] = (int8_t)msgs_sign_core<C>(sigs + (size_t)e * siglen, sig_type, hash_type,
+						      W_aff + (size_t)e * (2 * C::PLEN), x, k, msgs + off[e],
+						      off[e + 1] - off[e], pk, key_ok, id,
+						      idlen > kSm2MaxIdLen ? kSm2MaxIdLen + 1 : (uint32_t)idlen, ix);
+		if (e < T) break;
+	}
+}
+
 /* ------------------------------------------------------------------------------------------ Schnorr-family sign */
 
 /* H(tag) of BIP0340 tags tag0 .. tag0 + ntags - 1 into shared memory, one thread per tag: once per CTA, not per item */
@@ -1363,6 +1447,10 @@ template <class C> struct LaunchMisc {
 	static void schnorr_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *privkeys,
 				   const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
 				   const uint8_t *W_aff, uint8_t *sigs, int8_t *status, cudaStream_t st);
+	static void msgs_sign_finish(uint32_t blocks, uint32_t n, int sig_type, int hash_type, const uint8_t *privkeys,
+				     const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
+				     const uint8_t *ids, const uint64_t *id_off, const uint8_t *W_aff, uint32_t *prefix,
+				     uint8_t *sigs, int8_t *status, cudaStream_t st);
 	static void fp_mul(int which, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out, cudaStream_t st);
 	static void fp_addsub(int which, int op, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out,
 			      cudaStream_t st);
@@ -1466,6 +1554,15 @@ void LaunchMisc<C>::schnorr_finish(uint32_t n, int sig_type, int hash_type, cons
 {
 	k_schnorr_sign_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, sig_type, hash_type, privkeys, pubkeys, nonces, msgs,
 								    off, W_aff, sigs, status);
+}
+template <class C>
+void LaunchMisc<C>::msgs_sign_finish(uint32_t blocks, uint32_t n, int sig_type, int hash_type, const uint8_t *privkeys,
+				     const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
+				     const uint8_t *ids, const uint64_t *id_off, const uint8_t *W_aff, uint32_t *prefix,
+				     uint8_t *sigs, int8_t *status, cudaStream_t st)
+{
+	k_msgs_sign_finish<C><<<blocks, kThreads, 0, st>>>(n, sig_type, hash_type, privkeys, pubkeys, nonces, msgs, off, ids,
+							    id_off, W_aff, prefix, sigs, status);
 }
 template <class C>
 void LaunchMisc<C>::prj_unique(uint32_t blocks, uint32_t n, const uint8_t *prj, uint32_t *jac, uint32_t *prefix,

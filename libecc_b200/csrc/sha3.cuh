@@ -29,6 +29,17 @@ struct Seg2 { /* pre[0 .. npre) followed by msg */
 	const uint8_t *msg;
 	SHA3_HD uint32_t operator[](uint64_t i) const { return i < npre ? pre[i] : msg[i - npre]; }
 };
+struct Seg3 { /* pre[0 .. npre), then mid[0 .. nmid), then post: SM2's Z = H(ENTL || ID || a || b || G || Y) */
+	const uint8_t *pre;
+	uint32_t npre;
+	const uint8_t *mid;
+	uint64_t nmid;
+	const uint8_t *post;
+	SHA3_HD uint32_t operator[](uint64_t i) const
+	{
+		return i < npre ? pre[i] : (i - npre < nmid ? mid[i - npre] : post[i - npre - nmid]);
+	}
+};
 
 static SHA3_HD uint64_t rotl64_(uint64_t x, int n) { return n ? ((x << n) | (x >> (64 - n))) : x; }
 
