@@ -312,6 +312,45 @@ int eccb200_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, u
 /* Signature length in bytes of eccb200_sign_msgs_batch on this context's curve, or -1 (unsupported sig_type / hash). */
 int eccb200_sign_sig_len(eccb200_ctx *ctx, int sig_type, int hash_type);
 
+/*
+ * Batched ECKCDSA / ECSDSA / ECOSDSA / ECGDSA / ECRDSA / SM2 verification of raw messages, hashed on the device: one
+ * kernel for the signature checks, the hash and the mod-q scalars a, b; the double-scalar kernel W' = a*G + b*Y (as
+ * eccb200_double_smul_batch); one kernel for the acceptance test.  Y is the public key, each scheme as the reference's
+ * default build (ec_verify with the SM2 ID as ancillary data):
+ *   ECCB200_ALG_ECSDSA / _ECOSDSA  sig r || s, hsize + qlen bytes; s in ]0, q[, e = -(OS2I(r) mod q) != 0; a = s, b = e;
+ *                       accept iff H(W'_x || W'_y || m) (ECOSDSA: H(W'_x || m)) == r   (src/sig/ecsdsa_common.c:425-609)
+ *   ECCB200_ALG_ECKCDSA sig r || s, min(hsize, qlen) + qlen bytes; s in ]0, q[, z the first block-size bytes of
+ *                       Y_x || Y_y (zero-padded or cut), e = OS2I(r XOR rightmost(H(z || m))) mod q; a = e, b = s;
+ *                       accept iff the rightmost r_len bytes of H(W'_x) == r            (src/sig/eckcdsa.c:543-832)
+ *   ECCB200_ALG_ECGDSA  sig r || s, 2*qlen bytes; r, s in ]0, q[, e = leftmost bitlen(q) bits of H(m); a = r^-1 e,
+ *                       b = r^-1 s; accept iff W'_x mod q == r                           (src/sig/ecgdsa.c:413-600)
+ *   ECCB200_ALG_ECRDSA  sig r || s, 2*qlen bytes; r, s in ]0, q[, h = OS2I(byte-reversed H(m)) mod q, 0 replaced by 1;
+ *                       a = h^-1 s, b = -h^-1 r; accept iff W'_x mod q == r (not the ISO 14888-3 variant, which
+ *                       hashes without the byte reversal)                                (src/sig/ecrdsa.c:417-600)
+ *   ECCB200_ALG_SM2     sig r || s, 2*qlen bytes; r, s in ]0, q[, t = r + s mod q != 0; a = s, b = t; accept iff
+ *                       (OS2I(H(Z || m)) + W'_x) mod q == r, Z as in eccb200_sign_msgs_batch  (src/sig/sm2.c:518-700)
+ *   W' at infinity is invalid in every scheme.
+ *   sigs       : [n][siglen] with the lengths above (eccb200_sign_sig_len gives them for ECKCDSA / ECGDSA / ECRDSA /
+ *                SM2 only)
+ *   pubkeys    : n * 2*plen affine, every scheme; a key off the curve makes that item invalid
+ *   msgs / offsets, ids / id_offsets : as eccb200_sign_msgs_batch (the offsets are checked in the host form only); ids
+ *                are required for SM2 and ignored otherwise; an SM2 ID longer than 8191 bytes makes that item invalid
+ *                (the reference's sm2_compute_Z fails on it), in both forms
+ *   hash_type  : 2 .. 8 or 11 (SM3), for all six schemes
+ *   verdict    : per item 0 (valid) or -1 (invalid, or any error such as a key off the curve)
+ * Any other sig_type (ECDSA, ECFSDSA and BIP0340 have their own entry points), any other hash_type, or SM2 without ids
+ * returns -1 (eccb200_last_error) and writes nothing.  The _dev form follows the rules of every *_dev entry point (one
+ * scratch set per context, calls chained across streams; 16-byte alignment of d_sigs and d_pubkeys on the
+ * 256/384/512-bit curves, not of d_msgs or d_ids).
+ * NOTE: like every entry point of this library this is a throughput path, NOT a constant-time one.
+ */
+int eccb200_verify_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *sigs,
+			      const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *offsets, const uint8_t *ids,
+			      const uint64_t *id_offsets, int8_t *verdict);
+int eccb200_verify_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *d_sigs,
+				  const uint8_t *d_pubkeys, const uint8_t *d_msgs, const uint64_t *d_offsets,
+				  const uint8_t *d_ids, const uint64_t *d_id_offsets, int8_t *d_verdict, void *stream);
+
 /* cudaMemcpy device -> host (for callers that do not link the CUDA runtime). */
 int eccb200_copy_to_host(eccb200_ctx *ctx, void *host_dst, const void *d_src, size_t bytes);
 

@@ -42,7 +42,7 @@ ABI_SYMBOLS = [
     "eccb200_bip0340_verify_batch_dev", "eccb200_push_results", "eccb200_bind_thread_near_device",
     "eccb200_pipeline_chunk_bounds", "eccb200_double_smul_batch", "eccb200_double_smul_batch_dev",
     "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev", "eccb200_sign_msgs_batch",
-    "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len",
+    "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len", "eccb200_verify_msgs_batch", "eccb200_verify_msgs_batch_dev",
 ]
 
 _lib = None
@@ -128,6 +128,9 @@ def load_library() -> ctypes.CDLL:
     lib.eccb200_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, u8p, vp, u8p, vp,
                                                 u8p, i8p, vp]
     lib.eccb200_sign_sig_len.argtypes = [vp, ctypes.c_int, ctypes.c_int]
+    lib.eccb200_verify_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp, i8p]
+    lib.eccb200_verify_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp, i8p,
+                                                  vp]
     lib.eccb200_copy_to_host.argtypes = [vp, vp, vp, ctypes.c_size_t]
     lib.eccb200_bind_thread_near_device.argtypes = [ctypes.c_int]
     lib.eccb200_pipeline_chunk_bounds.argtypes = [u32, u32, u32, u32, ctypes.c_int, vp, ctypes.c_int]
@@ -427,6 +430,43 @@ class Engine:
             self._h, self.SIGN_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, d_privkeys.data_ptr(), ptr(d_pubkeys),
             d_nonces.data_ptr(), d_msgs.data_ptr(), d_offsets.data_ptr(), ptr(d_ids), ptr(d_id_offsets),
             d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_sign_msgs_batch_dev")
+
+    VERIFY_ALGS = {"ECKCDSA": 2, "ECSDSA": 3, "ECOSDSA": 4, "ECGDSA": 6, "ECRDSA": 7, "SM2": 8}  # ec_alg_type values
+
+    def verify_sig_len(self, alg: str, hash_name: str) -> int:
+        """signature length of verify_msgs_batch: hsize + qlen (ECSDSA, ECOSDSA), min(hsize, qlen) + qlen (ECKCDSA),
+        2*qlen (ECGDSA, ECRDSA, SM2)"""
+        if alg not in self.VERIFY_ALGS:
+            raise KeyError(alg)
+        hs = dict(self.HASH_LEN, SM3=32)[hash_name]
+        return {"ECSDSA": hs, "ECOSDSA": hs, "ECKCDSA": min(hs, self.qlen)}.get(alg, self.qlen) + self.qlen
+
+    def verify_msgs_batch(self, alg: str, hash_name: str, sigs, pubkeys, msgs, ids=None) -> np.ndarray:
+        """ECKCDSA / ECSDSA / ECOSDSA / ECGDSA / ECRDSA / SM2 verification of raw messages, hashed on the device
+        (hash_name may be "SM3").  sigs: n * verify_sig_len bytes, pubkeys: n * 2*plen affine, ids (a list of byte
+        strings, the SM2 user IDs) required for SM2.  Returns verdict[n]: 0 valid, -1 invalid."""
+        n = len(msgs)
+        sg = _as_u8(sigs, n * self.verify_sig_len(alg, hash_name))
+        pk = _as_u8(pubkeys, n * 2 * self.plen)
+        blob, off = self._pack_msgs(msgs)
+        id_blob, id_off = self._pack_msgs(ids) if ids is not None else (None, None)
+        verdict = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_verify_msgs_batch(
+            self._h, self.VERIFY_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, sg.ctypes.data, pk.ctypes.data,
+            blob.ctypes.data, off.ctypes.data, id_blob.ctypes.data if id_blob is not None else None,
+            id_off.ctypes.data if id_off is not None else None, verdict.ctypes.data), "eccb200_verify_msgs_batch")
+        return verdict
+
+    def verify_msgs_batch_dev(self, alg: str, hash_name: str, d_sigs, d_pubkeys, d_msgs, d_offsets, d_verdict,
+                              d_ids=None, d_id_offsets=None, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`); n = d_verdict.numel(); d_offsets / d_id_offsets:
+        n + 1 uint64 entries, not re-checked."""
+        n = d_verdict.numel()
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        self._check(self.lib.eccb200_verify_msgs_batch_dev(
+            self._h, self.VERIFY_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, d_sigs.data_ptr(), d_pubkeys.data_ptr(),
+            d_msgs.data_ptr(), d_offsets.data_ptr(), ptr(d_ids), ptr(d_id_offsets), d_verdict.data_ptr(),
+            ctypes.c_void_p(stream_handle)), "eccb200_verify_msgs_batch_dev")
 
     def copy_to_host(self, d_ptr: int, nbytes: int) -> np.ndarray:
         out = np.empty(nbytes, dtype=np.uint8)

@@ -1080,6 +1080,38 @@ template <class C> ECC_D void sm2_z(int hash_type, const uint8_t *id, uint32_t i
 	msg_hash_seg3(hash_type, Seg3{ ent, 2, id, idlen, tail }, 2 + (uint64_t)idlen + 6 * PL, Z);
 }
 
+/* SM2's e = OS2I(H(Z || m)) mod q (_sm2_sign_finalize step 5, _sm2_verify_finalize steps 2 and 5, sig/sm2.c:392,
+ * :649-666), Z from sm2_z.  Z and h are the caller's 64-byte buffers (the signer reuses its own: a separate frame
+ * here costs it registers). */
+template <class C>
+ECC_D void sm2_digest_scalar(Fe<C::N> &e, int hash_type, const uint8_t *id, uint32_t idlen, const uint8_t *Y,
+			     const uint8_t *msg, uint64_t mlen, uint8_t *Z, uint8_t *h)
+{
+	const int ds = msg_hash_digest_size(hash_type);
+	sm2_z<C>(hash_type, id, idlen, Y, Z);
+	msg_hash_seg3(hash_type, Seg3{ Z, (uint32_t)ds, msg, mlen, nullptr }, (uint64_t)ds + mlen, h);
+	digest_full_mod_q<C>(e, h, (uint32_t)ds);
+}
+
+/* ECKCDSA's H(z || m), z the first block-size bytes of Y_x || Y_y || 0... (z_len = block_size, sig/eckcdsa.c:223 sign,
+ * :578-625 verify); Y is the affine wire key, z the caller's kMsgsMaxPrefix-byte buffer, h receives the whole digest */
+template <class C>
+ECC_D void eckcdsa_hash_zm(int hash_type, const uint8_t *Y, const uint8_t *msg, uint64_t mlen, uint8_t *z, uint8_t *h)
+{
+	const int bs = msg_hash_block_size(hash_type);
+	for (int i = 0; i < bs; i++) z[i] = i < 2 * C::PLEN ? Y[i] : 0u;
+	msg_hash_seg3(hash_type, Seg3{ z, (uint32_t)bs, msg, mlen, nullptr }, (uint64_t)bs + mlen, h);
+}
+
+/* ECRDSA's scalar of the digest h = H(m): OS2I(byte-reversed h) mod q, 0 replaced by 1 (sig/ecrdsa.c:297-313 sign,
+ * :546-555 verify); rev is the caller's 64-byte buffer */
+template <class C> ECC_HD void ecrdsa_digest_scalar(Fe<C::N> &e, const uint8_t *h, int ds, uint8_t *rev)
+{
+	for (int i = 0; i < ds; i++) rev[i] = h[ds - 1 - i];
+	digest_full_mod_q<C>(e, rev, (uint32_t)ds);
+	if (Field<typename C::Fq>::is_zero(e)) e.w[0] = 1;
+}
+
 /*
  * One ECKCDSA / ECGDSA / ECRDSA / SM2 signature from W = k*G (affine wire bytes, as K4 writes them), the private scalar
  * x and the nonce k (plain integers) and the message (in memory, read where it lies).  Every scheme follows the
@@ -1119,11 +1151,9 @@ ECC_D int msgs_sign_core(uint8_t *sig, int sig_type, int hash_type, const uint8_
 	bool retry = false;
 	int rlen = QL, shift = 0;
 	if (sig_type == SIG_ECKCDSA) {
-		const int bs = msg_hash_block_size(hash_type);
-		for (int i = 0; i < bs; i++) pre[i] = i < 2 * PL ? Y[i] : 0u;
 		uint8_t hr[64];
-		msg_hash_seg3(hash_type, Seg3{ pre, (uint32_t)bs, msg, mlen, nullptr }, (uint64_t)bs + mlen, h); /* H(z || m) */
-		msg_hash_seg3(hash_type, Seg3{ W, (uint32_t)PL, nullptr, 0, nullptr }, (uint64_t)PL, hr);      /* H(W_x)    */
+		eckcdsa_hash_zm<C>(hash_type, Y, msg, mlen, pre, h);                                       /* H(z || m) */
+		msg_hash_seg3(hash_type, Seg3{ W, (uint32_t)PL, nullptr, 0, nullptr }, (uint64_t)PL, hr); /* H(W_x)    */
 		rlen = ds < QL ? ds : QL;
 		shift = ds - rlen;
 		for (int i = 0; i < rlen; i++) {
@@ -1134,9 +1164,7 @@ ECC_D int msgs_sign_core(uint8_t *sig, int sig_type, int hash_type, const uint8_
 		Fq::sub(t, k, e);
 		Fq::mul(s, t, xm); /* x*(k - e) */
 	} else if (sm2) {
-		sm2_z<C>(hash_type, id, idlen, Y, pre);
-		msg_hash_seg3(hash_type, Seg3{ pre, (uint32_t)ds, msg, mlen, nullptr }, (uint64_t)ds + mlen, h);
-		digest_full_mod_q<C>(e, h, (uint32_t)ds);
+		sm2_digest_scalar<C>(e, hash_type, id, idlen, Y, msg, mlen, pre, h);
 		Fq::add(r, e, r);  /* (OS2I(H) + W_x) mod q */
 		retry = Fq::is_zero(r);
 		Fq::mul(t, r, xm); /* r*x */
@@ -1152,9 +1180,7 @@ ECC_D int msgs_sign_core(uint8_t *sig, int sig_type, int hash_type, const uint8_
 			Fq::add(t, t, e);
 			Fq::mul(s, t, xm);
 		} else {
-			for (int i = 0; i < ds; i++) pre[i] = h[ds - 1 - i];
-			digest_full_mod_q<C>(e, pre, (uint32_t)ds);
-			if (Fq::is_zero(e)) e.w[0] = 1;
+			ecrdsa_digest_scalar<C>(e, h, ds, pre);
 			Fq::mul(t, r, xm); /* r*x */
 			Fq::mul(s, e, km); /* k*e */
 			Fq::add(s, s, t);
@@ -1189,6 +1215,144 @@ ECC_HD int ecdsa_verify_core(const Fe<C::N> &r, const Fe<C::N> &s, const Fe<C::N
 	Fe<C::N> u, v;
 	ecdsa_uv<C>(u, v, r, s, e);
 	return ecdsa_verify_tail<C>(r, u, v, Y, table, w);
+}
+
+/* ---------------------------------------- message verifiers (ECKCDSA, ECSDSA, ECOSDSA, ECGDSA, ECRDSA, SM2) */
+
+/* r || s: hsize + qlen (ECSDSA / ECOSDSA), min(hsize, qlen) + qlen (ECKCDSA), 2*qlen (ECGDSA, ECRDSA, SM2) */
+template <class C> ECC_HD int msgs_verify_sig_len(int sig_type, int digest_size)
+{
+	return sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA ? digest_size + C::QLEN :
+								   msgs_sig_len<C>(sig_type, digest_size);
+}
+
+/* ECGDSA (r^-1) and ECRDSA (h^-1) need one inversion mod q per item to form their scalars */
+ECC_HD bool msgs_verify_inverts(int sig_type) { return sig_type == SIG_ECGDSA || sig_type == SIG_ECRDSA; }
+
+/*
+ * First half of one verification, before W' = a*G + b*Y: the signature checks, the hash of the message and the mod-q
+ * scalars (plain integers < q), each scheme as the reference's default build (the drop-in's DsScheme objects restate
+ * the same rules):
+ *   ECSDSA / ECOSDSA  s in ]0, q[, e = -(OS2I(r) mod q) != 0; a = s, b = e     (sig/ecsdsa_common.c:475-498)
+ *   ECKCDSA           s in ]0, q[, e = OS2I(r XOR rightmost r_len bytes of H(z || m)) mod q; a = e, b = s
+ *                                                                              (sig/eckcdsa.c:592-773)
+ *   ECGDSA            r, s in ]0, q[, e = leftmost bitlen(q) bits of H(m); a = e, b = s, den = r
+ *                                                                              (sig/ecgdsa.c:451-568)
+ *   ECRDSA            r, s in ]0, q[, h = ecrdsa_digest_scalar(H(m)); a = s, b = -r, den = h
+ *                     (the reference never range-checks r, sig/ecrdsa.c:448-449; an r >= q fails its final comparison
+ *                     with r' < q, so refusing it here gives the same verdict)  (:546-569)
+ *   SM2               r, s in ]0, q[, t = r + s mod q != 0, ID at most 8191 bytes; a = s, b = t  (sig/sm2.c:553-671)
+ * For ECGDSA and ECRDSA a and b are still to be multiplied by den^-1 (msgs_verify_scale); den is 0 for the other
+ * schemes.  Y is the affine wire key (read by ECKCDSA only).  Returns false (a = b = den = 0) when the reference
+ * rejects the item before W'; a valid item never has a = b = 0, because s != 0 is one of its scalars.
+ */
+template <class C>
+ECC_D bool msgs_verify_prep_core(int sig_type, int hash_type, const uint8_t *sig, const uint8_t *Y, const uint8_t *msg,
+				 uint64_t mlen, uint32_t idlen, Fe<C::N> &a, Fe<C::N> &b, Fe<C::N> &den)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, QL = C::QLEN;
+	const int ds = msg_hash_digest_size(hash_type);
+	Fq::set_zero(a);
+	Fq::set_zero(b);
+	Fq::set_zero(den);
+	Fe<N> r, s;
+	uint8_t pre[kMsgsMaxPrefix], h[64];
+	if (sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA) {
+		load_be<N>(s, sig + ds, QL);
+		if (Fq::is_zero(s) || Fq::geq_mod(s)) return false;
+		digest_full_mod_q<C>(r, sig, (uint32_t)ds);
+		if (Fq::is_zero(r)) return false;
+		a = s;
+		Fq::neg(b, r);
+		return true;
+	}
+	if (sig_type == SIG_ECKCDSA) {
+		const int rlen = ds < QL ? ds : QL, shift = ds - rlen;
+		load_be<N>(s, sig + rlen, QL);
+		if (Fq::is_zero(s) || Fq::geq_mod(s)) return false;
+		eckcdsa_hash_zm<C>(hash_type, Y, msg, mlen, pre, h);
+		for (int i = 0; i < rlen; i++) h[i] = h[shift + i] ^ sig[i];
+		digest_full_mod_q<C>(a, h, (uint32_t)rlen);
+		b = s;
+		return true;
+	}
+	load_be<N>(r, sig, QL);
+	load_be<N>(s, sig + QL, QL);
+	if (!ecdsa_rs_in_range<C>(r, s)) return false;
+	if (sig_type == SIG_SM2) {
+		Fe<N> t;
+		Fq::add(t, r, s);
+		if (idlen > kSm2MaxIdLen || Fq::is_zero(t)) return false;
+		a = s;
+		b = t;
+		return true;
+	}
+	msg_hash_seg3(hash_type, Seg3{ nullptr, 0, msg, mlen, nullptr }, mlen, h);
+	if (sig_type == SIG_ECGDSA) {
+		digest_to_scalar<C>(a, h, (uint32_t)ds);
+		b = s;
+		den = r;
+	} else {
+		ecrdsa_digest_scalar<C>(den, h, ds, pre);
+		a = s;
+		Fq::neg(b, r);
+	}
+	return true;
+}
+
+/* ECGDSA / ECRDSA: a, b <- a * den^-1, b * den^-1 mod q, inv = den^-1 in the Montgomery domain of q */
+template <class C> ECC_HD void msgs_verify_scale(Fe<C::N> &a, Fe<C::N> &b, const Fe<C::N> &inv)
+{
+	typedef Field<typename C::Fq> Fq;
+	Fe<C::N> t;
+	Fq::mul(t, a, inv);
+	a = t;
+	Fq::mul(t, b, inv);
+	b = t;
+}
+
+/*
+ * Second half, after a finite W' (affine wire bytes): the scheme's acceptance test.
+ *   ECSDSA / ECOSDSA  H(W'_x || W'_y || m) resp. H(W'_x || m) == r      (sig/ecsdsa_common.c:500-520, :606)
+ *   ECKCDSA           rightmost r_len bytes of H(W'_x) == r             (sig/eckcdsa.c:778-800)
+ *   ECGDSA / ECRDSA   W'_x mod q == r                                   (sig/ecgdsa.c:577-585, ecrdsa.c:580-585)
+ *   SM2               (OS2I(H(Z || m)) + W'_x) mod q == r               (sig/sm2.c:664-688)
+ * Y is the affine wire key (SM2's Z), id / idlen SM2's ID (at most 8191 bytes: the prep refused longer ones).
+ */
+template <class C>
+ECC_D bool msgs_verify_accept(int sig_type, int hash_type, const uint8_t *sig, const uint8_t *W, const uint8_t *Y,
+			      const uint8_t *msg, uint64_t mlen, const uint8_t *id, uint32_t idlen)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, PL = C::PLEN, QL = C::QLEN;
+	const int ds = msg_hash_digest_size(hash_type);
+	uint8_t h[64];
+	if (sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA) {
+		const uint32_t nw = sig_type == SIG_ECSDSA ? 2 * PL : PL;
+		msg_hash_seg3(hash_type, Seg3{ W, nw, msg, mlen, nullptr }, (uint64_t)nw + mlen, h);
+		uint8_t diff = 0;
+		for (int i = 0; i < ds; i++) diff |= h[i] ^ sig[i];
+		return diff == 0;
+	}
+	if (sig_type == SIG_ECKCDSA) {
+		const int rlen = ds < QL ? ds : QL, shift = ds - rlen;
+		msg_hash_seg3(hash_type, Seg3{ W, (uint32_t)PL, nullptr, 0, nullptr }, (uint64_t)PL, h);
+		uint8_t diff = 0;
+		for (int i = 0; i < rlen; i++) diff |= h[shift + i] ^ sig[i];
+		return diff == 0;
+	}
+	Fe<N> x, r;
+	load_be<N>(x, W, PL);
+	scalar_reduce<C>(x); /* W'_x mod q */
+	load_be<N>(r, sig, QL);
+	if (sig_type == SIG_SM2) {
+		Fe<N> e;
+		uint8_t Z[64];
+		sm2_digest_scalar<C>(e, hash_type, id, idlen, Y, msg, mlen, Z, h);
+		Fq::add(x, x, e);
+	}
+	return Fq::eq(x, r);
 }
 
 } // namespace eccb200

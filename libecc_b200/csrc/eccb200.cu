@@ -1701,10 +1701,10 @@ struct SignChunk {
 	int8_t *status;
 };
 
-/* Host-pointer form of the message signers (Schnorr family and the others): chunks of four waves on two streams like
- * eccb200_ecdsa_verify_msgs_batch (a chunk's copies overlap the other chunk's kernels), K1 / K4 scratch from the
- * per-stream stage buffers.  launch(s, cnt, chunk) queues one chunk's kernels on ctx->streams[s].  The caller has
- * checked the offsets. */
+/* Host-pointer form of the message signers (Schnorr family and the others) and of the message verifier: chunks of four
+ * waves on two streams like eccb200_ecdsa_verify_msgs_batch (a chunk's copies overlap the other chunk's kernels), K1 /
+ * K4 scratch from the per-stream stage buffers.  launch(s, cnt, chunk) queues one chunk's kernels on ctx->streams[s].
+ * siglen == 0 (the verifier): the status column is the only output.  The caller has checked the offsets. */
 template <class Launch>
 static int sign_msgs_pipeline(eccb200_ctx *ctx, uint32_t n, const SignCol (&cols)[3], size_t scratch_width,
 			      const SignRagged (&rag)[2], size_t siglen, uint8_t *sigs, int8_t *status, Launch launch)
@@ -1770,7 +1770,8 @@ static int sign_msgs_pipeline(eccb200_ctx *ctx, uint32_t n, const SignCol (&cols
 			break;
 		}
 		rc = launch(s, cnt, ch);
-		if (!rc && (cudaMemcpyAsync(sigs + lo * siglen, ch.sigs, cnt * siglen, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+		if (!rc && ((siglen && cudaMemcpyAsync(sigs + lo * siglen, ch.sigs, cnt * siglen, cudaMemcpyDeviceToHost, st) !=
+						cudaSuccess) ||
 			    cudaMemcpyAsync(status + lo, ch.status, cnt, cudaMemcpyDeviceToHost, st) != cudaSuccess))
 			rc = fail("D2H copy failed");
 	}
@@ -1922,6 +1923,100 @@ extern "C" int eccb200_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_
 							       ch.sigs, ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
 							       ctx->stage_aff[s], ctx->streams[s]);
 				  });
+}
+
+/* -------------------------------------------- ECKCDSA / ECSDSA / ECOSDSA / ECGDSA / ECRDSA / SM2 verification */
+
+static const char *kVerifyAlgMsg =
+	"unsupported sig_type (ECKCDSA = 2, ECSDSA = 3, ECOSDSA = 4, ECGDSA = 6, ECRDSA = 7, SM2 = 8)";
+static bool verify_msgs_alg_ok(int sig_type)
+{
+	return msgs_alg_ok(sig_type) || sig_type == SIG_ECSDSA || sig_type == SIG_ECOSDSA;
+}
+
+/* the checks both forms share; 0, or -1 with the reason in eccb200_last_error */
+static int msgs_verify_args(const eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const void *sigs,
+			    const void *pubkeys, const void *offsets, const void *ids, const void *id_offsets,
+			    const void *verdict)
+{
+	if (!ctx) return fail("null argument");
+	if (!verify_msgs_alg_ok(sig_type)) return fail(kVerifyAlgMsg);
+	if (!msg_hash_digest_size(hash_type)) return fail(kMsgsHashMsg);
+	if (n && (!sigs || !pubkeys || !offsets || !verdict || (sig_type == SIG_SM2 && (!ids || !id_offsets))))
+		return fail("null argument");
+	return 0;
+}
+
+/* prep kernel (checks, hash, a || b into jac), the double-scalar kernel (W' into aff, its status into d_verdict), finish
+ * kernel (acceptance test) — all on `st`.  The prep of ECGDSA / ECRDSA runs on the normalisation's grid (several items
+ * per thread share the CTA-wide inversion; den goes to aff, which W' overwrites later); the other schemes invert nothing
+ * and run one item per thread. */
+static int msgs_verify_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *d_sigs,
+			   const uint8_t *d_pub, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_ids,
+			   const uint64_t *d_id_off, int8_t *d_verdict, uint32_t *jac, uint32_t *prefix, uint8_t *aff,
+			   cudaStream_t st)
+{
+	if (n == 0) return 0;
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		/* [n][2*qlen] bytes fit the [n][3N] words of the Jacobian scratch, [n][N] words the [n][2*plen] bytes of aff */
+		static_assert(2 * C::QLEN <= 12 * C::N && 4 * C::N <= 2 * C::PLEN, "verify scratch layout");
+		uint8_t *ab = reinterpret_cast<uint8_t *>(jac);
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		LaunchMisc<C>::msgs_verify_prep(msgs_verify_inverts(sig_type) ? affine_grid(ctx, n) : grid_for(n), n, sig_type,
+						hash_type, d_sigs, d_pub, d_msgs, d_off, d_id_off, prefix,
+						reinterpret_cast<uint32_t *>(aff), ab, st);           /* checks, a || b */
+		LaunchVerify<C>::double_smul(n, ab, d_pub, ctx->table, ctx->w, aff, d_verdict, st); /* W' = aG + bY */
+		LaunchMisc<C>::msgs_verify_finish(n, sig_type, hash_type, d_sigs, d_pub, d_msgs, d_off, d_ids, d_id_off, aff,
+						  d_verdict, st);                                       /* accept */
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 3;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+extern "C" int eccb200_verify_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					     const uint8_t *d_sigs, const uint8_t *d_pubkeys, const uint8_t *d_msgs,
+					     const uint64_t *d_offsets, const uint8_t *d_ids, const uint64_t *d_id_offsets,
+					     int8_t *d_verdict, void *stream)
+{
+	if (msgs_verify_args(ctx, sig_type, hash_type, n, d_sigs, d_pubkeys, d_offsets, d_ids, d_id_offsets, d_verdict))
+		return -1;
+	if (misaligned16(ctx, { d_sigs, d_pubkeys })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_work(ctx, n)) return -1;
+	const bool sm2 = sig_type == SIG_SM2;
+	return msgs_verify_dev(ctx, sig_type, hash_type, n, d_sigs, d_pubkeys, d_msgs, d_offsets, sm2 ? d_ids : nullptr,
+			       sm2 ? d_id_offsets : nullptr, d_verdict, ctx->jac, ctx->prefix, ctx->aff,
+			       (cudaStream_t)stream);
+}
+
+/* Host-pointer form through sign_msgs_pipeline: signatures and keys are its columns, messages and IDs its ragged
+ * inputs, the verdicts its status column. */
+extern "C" int eccb200_verify_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *sigs,
+					 const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *offsets,
+					 const uint8_t *ids, const uint64_t *id_offsets, int8_t *verdict)
+{
+	if (msgs_verify_args(ctx, sig_type, hash_type, n, sigs, pubkeys, offsets, ids, id_offsets, verdict)) return -1;
+	if (n == 0) return 0;
+	const bool sm2 = sig_type == SIG_SM2;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	if (sm2 && !offsets_ok(id_offsets, n)) return fail("id_offsets must start at 0 and be non-decreasing");
+	size_t siglen = 0;
+	dispatch(ctx->curve_id, [&](auto c) {
+		siglen = (size_t)msgs_verify_sig_len<decltype(c)>(sig_type, msg_hash_digest_size(hash_type));
+		return 0;
+	});
+	const SignCol cols[3] = { { sigs, siglen }, { pubkeys, 2 * (size_t)ctx->plen }, { nullptr, 0 } };
+	const SignRagged rag[2] = { { msgs, offsets }, { sm2 ? ids : nullptr, sm2 ? id_offsets : nullptr } };
+	return sign_msgs_pipeline(ctx, n, cols, 0, rag, 0, nullptr, verdict, [&](int s, uint32_t cnt, const SignChunk &ch) {
+		return msgs_verify_dev(ctx, sig_type, hash_type, cnt, ch.col[0], ch.col[1], ch.rag_base[0], ch.rag_off[0],
+				       ch.rag_base[1], ch.rag_off[1], ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
+				       ctx->stage_aff[s], ctx->streams[s]);
+	});
 }
 
 /* cudaMemcpy device -> host for callers that do not link the CUDA runtime (bench.py reads peer-written buffers). */

@@ -1153,6 +1153,113 @@ __global__ void __launch_bounds__(128) k_msgs_sign_finish(uint32_t n, int sig_ty
 	}
 }
 
+/* ------------------------------------------------- ECKCDSA / ECSDSA / ECOSDSA / ECGDSA / ECRDSA / SM2 verify */
+
+/*
+ * First of the three launches of a message verification: per item the signature checks, the hash of the message and
+ * the scalars a || b of W' = a*G + b*Y (msgs_verify_prep_core), written to ab ([n][2*qlen], the double-scalar kernel's
+ * input).  A rejected item gets a = b = 0: W' is then infinity and the double-scalar kernel reports status 1 for it.
+ * ECGDSA and ECRDSA multiply by den^-1 (r^-1, h^-1) from the two-level simultaneous inversion of k_msgs_sign_finish: a
+ * serial prefix product over the thread's items (prefix scratch; den in the Montgomery domain in den_buf, 0 for a
+ * rejected item, which stays out of the product), one CTA-wide inversion, then the items in reverse order.  The other
+ * schemes invert nothing and run one item per thread.  Messages as k_sha2_batch; id_off: SM2's ID lengths only.
+ */
+template <class C>
+__global__ void __launch_bounds__(128) k_msgs_verify_prep(uint32_t n, int sig_type, int hash_type,
+							  const uint8_t *__restrict__ sigs,
+							  const uint8_t *__restrict__ pubkeys,
+							  const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+							  const uint64_t *__restrict__ id_off, uint32_t *__restrict__ prefix,
+							  uint32_t *__restrict__ den_buf, uint8_t *__restrict__ ab)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, QL = C::QLEN;
+	const bool inverting = msgs_verify_inverts(sig_type);
+	const uint32_t T = gridDim.x * blockDim.x;
+	const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+	const bool active = tid < n;
+	const int siglen = msgs_verify_sig_len<C>(sig_type, msg_hash_digest_size(hash_type));
+	Fe<N> acc;
+	Fq::set_one(acc);
+	uint32_t last = tid;
+	if (active) {
+		for (uint32_t e = tid; e < n; e += T) {
+			Fe<N> a, b, den;
+			const uint64_t idlen = id_off ? id_off[e + 1] - id_off[e] : 0;
+			const bool ok = msgs_verify_prep_core<C>(sig_type, hash_type, sigs + (size_t)e * siglen,
+								 pubkeys + (size_t)e * (2 * C::PLEN), msgs + off[e],
+								 off[e + 1] - off[e],
+								 idlen > kSm2MaxIdLen ? kSm2MaxIdLen + 1 : (uint32_t)idlen,
+								 a, b, den);
+			store_wire<N, QL>(ab + (size_t)e * (2 * QL), a);
+			store_wire<N, QL>(ab + (size_t)e * (2 * QL) + QL, b);
+			if (inverting) {
+				Fe<N> dm, t;
+				store_words<N>(prefix + (size_t)e * N, acc);
+				Fq::set_zero(dm);
+				if (ok) {
+					Fq::to_mont(dm, den);
+					Fq::mul(t, acc, dm);
+					acc = t;
+				}
+				store_words<N>(den_buf + (size_t)e * N, dm);
+			}
+			last = e;
+			if (n - e <= T) break;
+		}
+	}
+	if (!inverting) return; /* uniform: sig_type is the same for the whole grid */
+	Fe<N> inv;
+	__shared__ uint32_t sh_inv[ECC_CTA_INV_WORDS(N)];
+	cta_inverse_128<typename C::Fq>(inv, acc, sh_inv);
+	if (!active) return;
+	for (uint32_t e = last;; e -= T) {
+		Fe<N> dm;
+		load_words<N>(dm, den_buf + (size_t)e * N);
+		if (!Fq::is_zero(dm)) {
+			Fe<N> pre, di, t, a, b;
+			load_words<N>(pre, prefix + (size_t)e * N);
+			Fq::mul(di, inv, pre); /* den^-1 in Montgomery form */
+			Fq::mul(t, inv, dm);
+			inv = t;
+			load_wire<N, QL>(a, ab + (size_t)e * (2 * QL));
+			load_wire<N, QL>(b, ab + (size_t)e * (2 * QL) + QL);
+			msgs_verify_scale<C>(a, b, di);
+			store_wire<N, QL>(ab + (size_t)e * (2 * QL), a);
+			store_wire<N, QL>(ab + (size_t)e * (2 * QL) + QL, b);
+		}
+		if (e < T) break;
+	}
+}
+
+/*
+ * Last launch, one item per thread: verdict holds the double-scalar kernel's status (0 W' finite, 1 infinity, -1 key
+ * off the curve) and W_aff its affine W'.  Status 0 and the scheme's acceptance test (msgs_verify_accept: the hash of
+ * W' || m for ECSDSA / ECOSDSA, of W'_x for ECKCDSA, SM2's Z and H(Z || m)) give 0; anything else gives -1.
+ */
+template <class C>
+__global__ void __launch_bounds__(128) k_msgs_verify_finish(uint32_t n, int sig_type, int hash_type,
+							    const uint8_t *__restrict__ sigs,
+							    const uint8_t *__restrict__ pubkeys,
+							    const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+							    const uint8_t *__restrict__ ids,
+							    const uint64_t *__restrict__ id_off,
+							    const uint8_t *__restrict__ W_aff, int8_t *__restrict__ verdict)
+{
+	const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+	if (e >= n) return;
+	bool ok = verdict[e] == 0;
+	if (ok) {
+		const int siglen = msgs_verify_sig_len<C>(sig_type, msg_hash_digest_size(hash_type));
+		const uint64_t idlen = ids ? id_off[e + 1] - id_off[e] : 0;
+		ok = msgs_verify_accept<C>(sig_type, hash_type, sigs + (size_t)e * siglen, W_aff + (size_t)e * (2 * C::PLEN),
+					   pubkeys + (size_t)e * (2 * C::PLEN), msgs + off[e], off[e + 1] - off[e],
+					   ids ? ids + id_off[e] : nullptr,
+					   idlen > kSm2MaxIdLen ? kSm2MaxIdLen : (uint32_t)idlen);
+	}
+	verdict[e] = ok ? 0 : -1;
+}
+
 /* ------------------------------------------------------------------------------------------ Schnorr-family sign */
 
 /* H(tag) of BIP0340 tags tag0 .. tag0 + ntags - 1 into shared memory, one thread per tag: once per CTA, not per item */
@@ -1451,6 +1558,12 @@ template <class C> struct LaunchMisc {
 				     const uint8_t *pubkeys, const uint8_t *nonces, const uint8_t *msgs, const uint64_t *off,
 				     const uint8_t *ids, const uint64_t *id_off, const uint8_t *W_aff, uint32_t *prefix,
 				     uint8_t *sigs, int8_t *status, cudaStream_t st);
+	static void msgs_verify_prep(uint32_t blocks, uint32_t n, int sig_type, int hash_type, const uint8_t *sigs,
+				     const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *off, const uint64_t *id_off,
+				     uint32_t *prefix, uint32_t *den, uint8_t *ab, cudaStream_t st);
+	static void msgs_verify_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *sigs, const uint8_t *pubkeys,
+				       const uint8_t *msgs, const uint64_t *off, const uint8_t *ids, const uint64_t *id_off,
+				       const uint8_t *W_aff, int8_t *verdict, cudaStream_t st);
 	static void fp_mul(int which, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out, cudaStream_t st);
 	static void fp_addsub(int which, int op, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out,
 			      cudaStream_t st);
@@ -1563,6 +1676,22 @@ void LaunchMisc<C>::msgs_sign_finish(uint32_t blocks, uint32_t n, int sig_type, 
 {
 	k_msgs_sign_finish<C><<<blocks, kThreads, 0, st>>>(n, sig_type, hash_type, privkeys, pubkeys, nonces, msgs, off, ids,
 							    id_off, W_aff, prefix, sigs, status);
+}
+template <class C>
+void LaunchMisc<C>::msgs_verify_prep(uint32_t blocks, uint32_t n, int sig_type, int hash_type, const uint8_t *sigs,
+				     const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *off, const uint64_t *id_off,
+				     uint32_t *prefix, uint32_t *den, uint8_t *ab, cudaStream_t st)
+{
+	k_msgs_verify_prep<C><<<blocks, kThreads, 0, st>>>(n, sig_type, hash_type, sigs, pubkeys, msgs, off, id_off, prefix,
+							    den, ab);
+}
+template <class C>
+void LaunchMisc<C>::msgs_verify_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *sigs,
+				       const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *off, const uint8_t *ids,
+				       const uint64_t *id_off, const uint8_t *W_aff, int8_t *verdict, cudaStream_t st)
+{
+	k_msgs_verify_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, sig_type, hash_type, sigs, pubkeys, msgs, off, ids,
+								   id_off, W_aff, verdict);
 }
 template <class C>
 void LaunchMisc<C>::prj_unique(uint32_t blocks, uint32_t n, const uint8_t *prj, uint32_t *jac, uint32_t *prefix,
