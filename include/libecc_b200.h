@@ -177,6 +177,29 @@ int eccb200_ecdsa_verify_keystate_batch(eccb200_ctx *ctx, uint32_t n, const uint
 					int8_t *verdict);
 
 /*
+ * Batched ECDSA public-key recovery on pre-hashed messages: __ecdsa_public_key_from_sig per item
+ * (src/sig/ecdsa_common.c:867-1011, behind ecdsa_public_key_from_sig src/sig/ecdsa.c:73 and
+ * decdsa_public_key_from_sig src/sig/decdsa.c; the key type changes nothing in the computation).
+ *   sigs    : n * 2*qlen bytes r||s;  digests : n * hlen bytes, hlen 1..128 (e as for verification, :942-950)
+ *   keys    : n * 2 * 2*plen bytes, affine Y1 = v*R1 + u*G then Y2 = v*R2 + u*G (:992-999) with R1 = (r, sqrt1),
+ *             R2 = (r, -sqrt1), sqrt1 the first root of the reference's fp_sqrt (src/fp/fp_sqrt.c),
+ *             u = -e/r and v = s/r mod q (:981-990); a key is zero unless its status is OK
+ *   status  : n * 2 bytes, one per key: ECCB200_OK / ECCB200_INFINITY (the reference returns that key as the point at
+ *             infinity without complaint); both ECCB200_ERR where the reference returns -1: r or s outside [1, q-1]
+ *             (:900-912), r >= p (fp_set_nn, :958; possible on FRP256V1 only), or r^3 + ar + b not a square (:959)
+ * Only x = r is tried.  The reference's restart (:914-931, :960-971) first tries r + 2q, never r + q, and can not succeed
+ * on the curves of this library (cofactor 1, so q > p/2: r + 2q >= p, which fp_set_nn refuses, src/fp/fp.c:213).  So a
+ * signature whose nonce point had x >= q gives ECCB200_ERR, or keys from x = r when that happens to be an x coordinate,
+ * exactly as the reference does; never the keys of x = r + q.  One kernel launch per chunk: one ECDSA verification's
+ * elliptic-curve work plus one point addition per item.  The _dev form runs on `stream`; on the 256-, 384- and 512-bit
+ * curves d_sigs and d_keys must be 16-byte aligned.
+ */
+int eccb200_ecdsa_recover_batch(eccb200_ctx *ctx, uint32_t n, const uint8_t *sigs, const uint8_t *digests, uint32_t hlen,
+				uint8_t *keys, int8_t *status);
+int eccb200_ecdsa_recover_batch_dev(eccb200_ctx *ctx, uint32_t n, const uint8_t *d_sigs, const uint8_t *d_digests,
+				    uint32_t hlen, uint8_t *d_keys, int8_t *d_status, void *stream);
+
+/*
  * Batched ECDSA signing on pre-hashed messages with caller-supplied nonces: replaces, per signature,
  * __ecdsa_sign_finalize steps 3-11 (src/sig/ecdsa_common.c:403-560): k*G (:479), prj_pt_unique (:481), r = x mod q,
  * s = k^-1 (e + r*d) mod q (:537-540).  The nonce comes from the caller exactly as the reference's signing context

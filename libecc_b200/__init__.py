@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "eccb200_pipeline_chunk_bounds", "eccb200_double_smul_batch", "eccb200_double_smul_batch_dev",
     "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev", "eccb200_sign_msgs_batch",
     "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len", "eccb200_verify_msgs_batch", "eccb200_verify_msgs_batch_dev",
+    "eccb200_ecdsa_recover_batch", "eccb200_ecdsa_recover_batch_dev",
 ]
 
 _lib = None
@@ -141,6 +142,8 @@ def load_library() -> ctypes.CDLL:
     lib.eccb200_double_smul_batch_dev.argtypes = [vp, u32, u8p, u8p, u8p, i8p, vp]
     lib.eccb200_bip0340_verify_batch_dev.argtypes = [vp, u32, u8p, u8p, u8p, u32, i8p, vp]
     lib.eccb200_ecdsa_verify_keystate_batch.argtypes = [vp, u32, u8p, u8p, i8p, u8p, u32, i8p]
+    lib.eccb200_ecdsa_recover_batch.argtypes = [vp, u32, u8p, u8p, u32, u8p, i8p]
+    lib.eccb200_ecdsa_recover_batch_dev.argtypes = [vp, u32, u8p, u8p, u32, u8p, i8p, vp]
     lib.eccb200_host_alloc.argtypes = [ctypes.c_size_t]
     lib.eccb200_host_alloc.restype = ctypes.c_void_p
     lib.eccb200_host_alloc_input.argtypes = [ctypes.c_size_t]
@@ -271,6 +274,21 @@ class Engine:
             self._h, n, sg.ctypes.data, pk.ctypes.data, dg.ctypes.data, hlen, verdict.ctypes.data),
             "eccb200_ecdsa_verify_batch")
         return verdict
+
+    def ecdsa_recover_batch(self, sigs, digests, hlen: int) -> Tuple[np.ndarray, np.ndarray]:
+        """ECDSA public-key recovery: sigs [n][2*qlen] = r || s, digests [n][hlen].  Returns (keys[n, 2, 2*plen] uint8:
+        affine Y1 then Y2, status[n, 2] int8: OK / INFINITY per key, ERR for both where the reference returns -1)."""
+        sg = _as_u8(sigs)
+        n = sg.size // (2 * self.qlen)
+        if sg.size != n * 2 * self.qlen:
+            raise ValueError("sigs length is not a multiple of 2*qlen")
+        dg = _as_u8(digests, n * hlen)
+        keys = np.zeros((n, 2, 2 * self.plen), dtype=np.uint8)
+        status = np.zeros((n, 2), dtype=np.int8)
+        self._check(self.lib.eccb200_ecdsa_recover_batch(self._h, n, sg.ctypes.data, dg.ctypes.data, hlen,
+                                                         keys.ctypes.data, status.ctypes.data),
+                    "eccb200_ecdsa_recover_batch")
+        return keys, status
 
     def ecdsa_verify_prj_batch(self, sigs, prj_pubkeys, digests, hlen: int) -> np.ndarray:
         """Public keys as X || Y || Z (homogeneous projective, 3*plen bytes each)."""
@@ -725,6 +743,13 @@ class Engine:
         self._check(self.lib.eccb200_ecdsa_verify_batch_dev(
             self._h, n, d_sigs.data_ptr(), d_pubkeys.data_ptr(), d_digests.data_ptr(), hlen,
             d_verdict.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_ecdsa_verify_batch_dev")
+
+    def ecdsa_recover_batch_dev(self, d_sigs, d_digests, hlen: int, d_keys, d_status, stream_handle: int = 0):
+        """d_sigs [n][2*qlen], d_digests [n][hlen] -> d_keys [n][2][2*plen], d_status [n][2] (CUDA tensors)."""
+        n = d_sigs.numel() // (2 * self.qlen)
+        self._check(self.lib.eccb200_ecdsa_recover_batch_dev(
+            self._h, n, d_sigs.data_ptr(), d_digests.data_ptr(), hlen, d_keys.data_ptr(), d_status.data_ptr(),
+            ctypes.c_void_p(stream_handle)), "eccb200_ecdsa_recover_batch_dev")
 
 
 class MultiEngine:

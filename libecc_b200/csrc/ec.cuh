@@ -1217,6 +1217,71 @@ ECC_HD int ecdsa_verify_core(const Fe<C::N> &r, const Fe<C::N> &s, const Fe<C::N
 	return ecdsa_verify_tail<C>(r, u, v, Y, table, w);
 }
 
+/* ------------------------------------------------------------------------------------- ECDSA public-key recovery */
+
+/*
+ * __ecdsa_public_key_from_sig (sig/ecdsa_common.c:867-1011) in pieces shared by the kernel (k_ecdsa_recover) and the
+ * host build of the tests.  Only x = r is ever tried: the reference's restart with r + k*q (:914-931, :960-971) can
+ * not succeed on a curve of cofactor 1 (r + 2q >= p exits, or fp_set_nn refuses it), so it always ends in -1.
+ */
+
+/* r, s in [1, q-1] (:900-912) and r < p, which fp_set_nn requires (:958; only FRP256V1 has q > p) */
+template <class C> ECC_HD bool ecdsa_recover_rs_ok(const Fe<C::N> &r, const Fe<C::N> &s)
+{
+	return ecdsa_rs_in_range<C>(r, s) && !Field<typename C::Fp>::geq_mod(r);
+}
+
+/* R1 = (r, sqrt1) with sqrt1 the first root of fp_sqrt (aff_pt_y_from_x, curves/aff_pt.c); false when
+ * r^3 + ar + b is not a square.  r < p. */
+template <class C> ECC_HD bool ecdsa_recover_point(Aff<C> &R, const Fe<C::N> &r, int *loops = nullptr)
+{
+	typedef Field<typename C::Fp> F;
+	Fe<C::N> alpha;
+	F::to_mont(R.x, r);
+	EC<C>::curve_rhs(alpha, R.x);
+	return F::sqrt(R.y, alpha, loops);
+}
+
+/* u = -e * r^-1 mod q, v = s * r^-1 mod q (plain form) from ri = r^-1 in the Montgomery domain of q (:981-990) */
+template <class C>
+ECC_HD void ecdsa_recover_uv(Fe<C::N> &u, Fe<C::N> &v, const Fe<C::N> &e, const Fe<C::N> &s, const Fe<C::N> &ri)
+{
+	typedef Field<typename C::Fq> Fq;
+	Fq::mul(u, e, ri);
+	Fq::neg(u, u); /* nn_mod_neg: 0 stays 0 */
+	Fq::mul(v, s, ri);
+}
+
+/* Y1 = v*R1 + uG and Y2 = v*R2 + uG = uG - v*R1 (:992-999) from uG and V = v*R1: one scalar multiplication for both
+ * keys.  add_full resolves uG = +-V and the points at infinity; either key may be the point at infinity. */
+template <class C> ECC_HD void ecdsa_recover_keys(Jac<C> &Y1, Jac<C> &Y2, const Jac<C> &uG, const Jac<C> &V)
+{
+	Jac<C> Vn;
+	EC<C>::neg(Vn, V);
+	EC<C>::add_full(Y1, uG, V);
+	EC<C>::add_full(Y2, uG, Vn);
+}
+
+/* The whole recovery of one item with a per-item inversion of r (host build of the tests; the kernel shares the
+ * inversions across its CTA).  Returns false where the reference returns -1. */
+template <class C>
+ECC_HD bool ecdsa_recover_core(Jac<C> &Y1, Jac<C> &Y2, const Fe<C::N> &r, const Fe<C::N> &s, const Fe<C::N> &e,
+			       const uint32_t *__restrict__ table, int w)
+{
+	typedef Field<typename C::Fq> Fq;
+	Aff<C> R;
+	if (!ecdsa_recover_rs_ok<C>(r, s) || !ecdsa_recover_point<C>(R, r)) return false;
+	Fe<C::N> rm, ri, u, v;
+	Fq::to_mont(rm, r);
+	Fq::inv(ri, rm);
+	ecdsa_recover_uv<C>(u, v, e, s, ri);
+	Jac<C> uG, V;
+	comb_mul<C>(uG, u, table, w);
+	window_mul<C>(V, v, R, nullptr, ThreadInverter<C>());
+	ecdsa_recover_keys<C>(Y1, Y2, uG, V);
+	return true;
+}
+
 /* ---------------------------------------- message verifiers (ECKCDSA, ECSDSA, ECOSDSA, ECGDSA, ECRDSA, SM2) */
 
 /* r || s: hsize + qlen (ECSDSA / ECOSDSA), min(hsize, qlen) + qlen (ECKCDSA), 2*qlen (ECGDSA, ECRDSA, SM2) */

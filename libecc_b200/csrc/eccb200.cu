@@ -719,6 +719,30 @@ extern "C" int eccb200_ecdsa_verify_batch_dev(eccb200_ctx *ctx, uint32_t n, cons
 	return verify_dev(ctx, n, d_sigs, d_pubkeys, d_digests, hlen, d_verdict, (cudaStream_t)stream);
 }
 
+static int recover_dev(eccb200_ctx *ctx, uint32_t n, const uint8_t *d_sigs, const uint8_t *d_digests, uint32_t hlen,
+		       uint8_t *d_keys, int8_t *d_status, cudaStream_t st)
+{
+	if (n == 0) return 0;
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		LaunchVerify<C>::recover(n, d_sigs, d_digests, hlen, ctx->table, ctx->w, d_keys, d_status, st);
+		ctx->launches += 1;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+extern "C" int eccb200_ecdsa_recover_batch_dev(eccb200_ctx *ctx, uint32_t n, const uint8_t *d_sigs,
+					       const uint8_t *d_digests, uint32_t hlen, uint8_t *d_keys, int8_t *d_status,
+					       void *stream)
+{
+	if (!ctx || (n && (!d_sigs || !d_digests || !d_keys || !d_status))) return fail("null argument");
+	if (hlen == 0 || hlen > 128) return fail("bad digest length");
+	if (misaligned16(ctx, { d_sigs, d_keys })) return fail(kAlignMsg);
+	CUDA_OK(cudaSetDevice(ctx->device));
+	return recover_dev(ctx, n, d_sigs, d_digests, hlen, d_keys, d_status, (cudaStream_t)stream);
+}
+
 static int ecfsdsa_dev(eccb200_ctx *ctx, uint32_t n, const uint8_t *d_sigs, const uint8_t *d_pubkeys,
 		       const uint8_t *d_digests, uint32_t hlen, int8_t *d_verdict, cudaStream_t st)
 {
@@ -1111,6 +1135,23 @@ extern "C" int eccb200_ecdsa_verify_batch(eccb200_ctx *ctx, uint32_t n, const ui
 		const uint8_t *d = ctx->d_in[s];
 		return verify_dev(ctx, cnt, d, d + (size_t)cnt * sg, d + (size_t)cnt * (sg + pk), hlen,
 				  (int8_t *)ctx->d_out[s], ctx->streams[s]);
+	});
+}
+
+extern "C" int eccb200_ecdsa_recover_batch(eccb200_ctx *ctx, uint32_t n, const uint8_t *sigs, const uint8_t *digests,
+					   uint32_t hlen, uint8_t *keys, int8_t *status)
+{
+	if (!ctx || (n && (!sigs || !digests || !keys || !status))) return fail("null argument");
+	if (hlen == 0 || hlen > 128) return fail("bad digest length");
+	if (n == 0) return 0;
+	const size_t sg = 2 * (size_t)ctx->qlen, kl = 4 * (size_t)ctx->plen;
+	/* the digest column goes last: it is the only one whose item size need not be a multiple of 16 */
+	std::vector<HostCol> in = { { (uint8_t *)sigs, sg, false }, { (uint8_t *)digests, hlen, false } };
+	std::vector<HostCol> outc = { { keys, kl, false }, { (uint8_t *)status, 2, false } };
+	return run_pipeline(ctx, n, in, outc, [&](int s, uint32_t cnt) {
+		const uint8_t *d = ctx->d_in[s];
+		return recover_dev(ctx, cnt, d, d + (size_t)cnt * sg, hlen, ctx->d_out[s],
+				   (int8_t *)(ctx->d_out[s] + (size_t)cnt * kl), ctx->streams[s]);
 	});
 }
 

@@ -520,7 +520,83 @@ template <class F> struct Field : FieldCore<F> {
 		return eq(chk, a);
 	}
 
+	/*
+	 * r = the root of a that the reference's fp_sqrt returns FIRST (fp/fp_sqrt.c; the second is m - r), when a is
+	 * a square; returns whether it is.  Montgomery in, Montgomery out; a == 0 gives 0 (:153-160).  Fp tags only.
+	 *   m = 3 mod 4 (SQRT_S == 1): a^((m+1)/4), the reference's shortcut (:184-193), by sqrt_3mod4;
+	 *   otherwise: Tonelli-Shanks restated step by step (:194-253) with the reference's constants, m - 1 = Q * 2^S and
+	 *   c = z^Q for z its smallest non-residue counting up from 0 (tools/gen_curve_constants.py).  Which root comes out
+	 *   depends on every factor the loop multiplies in, so the loop makes the reference's choices, not just any.
+	 * `loops` (optional) receives the number of trips through the main loop.  Not constant time, like the reference.
+	 */
+	static ECC_HD bool sqrt(E &r, const E &a, int *loops = nullptr)
+	{
+		if (loops) *loops = 0;
+		if (F::SQRT_S == 1) return sqrt_3mod4(r, a);
+		if (is_zero(a)) {
+			set_zero(r);
+			return true;
+		}
+		E x, t, c, b, tmp, one;
+		pow_sqrt_qh(x, a); /* a^((Q-1)/2) */
+		mul(r, x, a);      /* r = a^((Q+1)/2) (:201-203) */
+		mul(t, r, x);      /* t = a^Q (:204) */
+		set_one(one);
+		/* Legendre symbol (:162-166): a^((m-1)/2) = t^(2^(S-1)) must be 1 */
+		tmp = t;
+#pragma unroll 1
+		for (int k = 0; k < F::SQRT_S - 1; k++) sqr(tmp, tmp);
+		if (!eq(tmp, one)) return false;
+#pragma unroll
+		for (int i = 0; i < N; i++) c.w[i] = F::SQRT_C(i);
+		int m = F::SQRT_S;
+#pragma unroll 1
+		while (!eq(t, one)) { /* (:209-253) */
+			int i = 1;
+			sqr(tmp, t);
+#pragma unroll 1
+			while (!eq(tmp, one) && i < m) { /* lowest i in (0, m) with t^(2^i) == 1; exists because a is a square */
+				sqr(tmp, tmp);
+				i++;
+			}
+			b = c; /* b = c^(2^(m-i-1)) */
+#pragma unroll 1
+			for (int k = 0; k < m - i - 1; k++) sqr(b, b);
+			mul(r, r, b);
+			sqr(c, b);
+			mul(t, t, c);
+			m = i;
+			if (loops) ++*loops;
+		}
+		return true;
+	}
+
       private:
+	/* r = a^((Q-1)/2) for the Tonelli-Shanks constant SQRT_QH: 4-bit fixed window, as in sqrt_3mod4 */
+	static ECC_HD void pow_sqrt_qh(E &r, const E &a)
+	{
+		E tbl[16];
+		set_one(tbl[0]);
+		tbl[1] = a;
+#pragma unroll 1
+		for (int i = 2; i < 16; i++) mul(tbl[i], tbl[i - 1], a);
+		E acc;
+		set_one(acc);
+#pragma unroll 1
+		for (int wi = N - 1; wi >= 0; wi--) {
+			uint32_t ew = 0;
+#pragma unroll
+			for (int k = 0; k < N; k++) ew = (k == wi) ? F::SQRT_QH(k) : ew;
+#pragma unroll 1
+			for (int nb = 7; nb >= 0; nb--) {
+#pragma unroll 1
+				for (int q = 0; q < 4; q++) sqr(acc, acc);
+				mul(acc, acc, tbl[(ew >> (4 * nb)) & 15u]);
+			}
+		}
+		r = acc;
+	}
+
 	static ECC_HD uint32_t pm2_word(int i)
 	{
 		uint32_t v = 0;

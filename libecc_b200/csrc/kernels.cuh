@@ -983,6 +983,91 @@ __global__ void ECC_CLUSTER_ATTR __launch_bounds__(128, (C::N <= 8 ? ECC_MINB_VE
 #endif
 }
 
+/* ------------------------------------------------------------------------------------------ ECDSA key recovery */
+
+/*
+ * Batched ECDSA public-key recovery, __ecdsa_public_key_from_sig (sig/ecdsa_common.c:867-1011), one item per thread:
+ * sigs[i] = r || s (2*QLEN bytes), digests[i] hlen bytes -> keys[i] = Y1 || Y2 (affine, 2*PLEN bytes each) and
+ * status[i] = { s1, s2 }: 0 finite, 1 the point at infinity, -1 both where the reference returns -1.
+ *   - range checks and r < p (ecdsa_recover_rs_ok), e as for verification (digest_to_scalar, :942-950);
+ *   - r^-1 mod q for the whole CTA at once (one nn_modinv per item in the reference, :984); rejected items give 1;
+ *   - R1 = (r, sqrt1) with the reference's root (Field::sqrt), x = r only (ec.cuh);
+ *   - u*G through the comb, V = v*R1 through the signed window, then Y1 = uG + V and Y2 = uG - V: the EC work of ONE
+ *     verification plus one addition, where the reference runs three ladders;
+ *   - both keys normalised by one CTA-wide inversion of Z1*Z2 (Z taken as 1 at infinity).
+ * A rejected item walks the same code on u = v = 0 and the generator: every CTA-wide inversion stays collective.
+ */
+template <class C>
+__global__ void ECC_CLUSTER_ATTR __launch_bounds__(128, (C::N <= 8 ? ECC_MINB_VERIFY : (C::N <= 12 ? ECC_MINB_VERIFY_WIDE : 2))) k_ecdsa_recover(uint32_t n, const uint8_t *__restrict__ sigs,
+								const uint8_t *__restrict__ digests, uint32_t hlen,
+								const uint32_t *__restrict__ table, int w,
+								uint8_t *__restrict__ keys, int8_t *__restrict__ status)
+{
+	typedef Field<typename C::Fq> Fq;
+	typedef Field<typename C::Fp> F;
+	constexpr int N = C::N;
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	const bool active = idx < n;
+	const uint32_t i0 = active ? idx : 0; /* idle threads of the last CTA still join the CTA-wide inversions */
+	__shared__ uint32_t sh_inv[ECC_CTA_INV_WORDS(N)];
+	Fe<N> r, s, e;
+	load_wire<N, C::QLEN>(r, sigs + (size_t)i0 * (2 * C::QLEN));
+	load_wire<N, C::QLEN>(s, sigs + (size_t)i0 * (2 * C::QLEN) + C::QLEN);
+	const bool rs_ok = ecdsa_recover_rs_ok<C>(r, s);
+	Fe<N> rm, ri;
+	Fq::set_one(rm);
+	if (rs_ok) Fq::to_mont(rm, r);
+	cta_inverse_128<typename C::Fq, ECC_CLUSTER_INV>(ri, rm, sh_inv);
+	digest_to_scalar<C>(e, digests + (size_t)i0 * hlen, hlen);
+	Aff<C> R;
+	const bool ok = rs_ok && ecdsa_recover_point<C>(R, r);
+	Fe<N> u, v;
+	ecdsa_recover_uv<C>(u, v, e, s, ri);
+	if (!ok) {
+		Fq::set_zero(u);
+		Fq::set_zero(v);
+#pragma unroll
+		for (int j = 0; j < N; j++) {
+			R.x.w[j] = C::GX_MONT(j);
+			R.y.w[j] = C::GY_MONT(j);
+		}
+	}
+	Jac<C> uG, V, Y1, Y2;
+	comb_mul<C>(uG, u, table, w);
+	window_mul<C>(V, v, R, nullptr, [&](Fe<N> &o, const Fe<N> &a) {
+		cta_inverse_128<typename C::Fp, ECC_CLUSTER_INV>(o, a, sh_inv);
+	});
+	ecdsa_recover_keys<C>(Y1, Y2, uG, V);
+	const bool inf1 = EC<C>::is_inf(Y1), inf2 = EC<C>::is_inf(Y2);
+	Fe<N> z1 = Y1.Z, z2 = Y2.Z, z12, zi;
+	if (inf1) F::set_one(z1);
+	if (inf2) F::set_one(z2);
+	F::mul(z12, z1, z2);
+	cta_inverse_128<typename C::Fp, ECC_CLUSTER_INV>(zi, z12, sh_inv);
+	if (!active) return;
+	uint8_t *out = keys + (size_t)idx * (4 * C::PLEN);
+	/* 1/Z1 = zi * Z2, 1/Z2 = zi * Z1; 1/Z out of the Montgomery domain once, so X * zp^2 and Y * zp^3 come out plain */
+	auto put = [&](uint8_t *o, const Jac<C> &P, const Fe<N> &zo, bool fin) {
+		Fe<N> zk, zp, zk2, zk3, x, y;
+		F::mul(zk, zi, zo);
+		F::from_mont(zp, zk);
+		F::mul(zk2, zp, zk);
+		F::mul(zk3, zk2, zk);
+		F::mul(x, P.X, zk2);
+		F::mul(y, P.Y, zk3);
+		if (!fin) {
+			F::set_zero(x);
+			F::set_zero(y);
+		}
+		store_wire<N, C::PLEN>(o, x);
+		store_wire<N, C::PLEN>(o + C::PLEN, y);
+	};
+	put(out, Y1, z2, ok && !inf1);
+	put(out + 2 * C::PLEN, Y2, z1, ok && !inf2);
+	status[2 * (size_t)idx] = !ok ? (int8_t)-1 : (inf1 ? (int8_t)1 : (int8_t)0);
+	status[2 * (size_t)idx + 1] = !ok ? (int8_t)-1 : (inf2 ? (int8_t)1 : (int8_t)0);
+}
+
 /* ------------------------------------------------------------------------------------------ ECDSA sign (next row f.1) */
 
 /*
@@ -1584,6 +1669,8 @@ template <class C> struct LaunchVerify {
 				uint8_t *out, int8_t *status, cudaStream_t st);
 	static void uv(uint32_t n, const uint8_t *sigs, const uint8_t *digests, uint32_t hlen, uint8_t *out,
 		       cudaStream_t st);
+	static void recover(uint32_t n, const uint8_t *sigs, const uint8_t *digests, uint32_t hlen, const uint32_t *table,
+			    int w, uint8_t *keys, int8_t *status, cudaStream_t st);
 };
 
 #if defined(ECC_TU_FIXED)
@@ -1788,6 +1875,12 @@ void LaunchVerify<C>::uv(uint32_t n, const uint8_t *sigs, const uint8_t *digests
 			 cudaStream_t st)
 {
 	k_ecdsa_uv<C><<<grid_for(n), kThreads, 0, st>>>(n, sigs, digests, hlen, out);
+}
+template <class C>
+void LaunchVerify<C>::recover(uint32_t n, const uint8_t *sigs, const uint8_t *digests, uint32_t hlen,
+			      const uint32_t *table, int w, uint8_t *keys, int8_t *status, cudaStream_t st)
+{
+	k_ecdsa_recover<C><<<grid_clustered(n), kThreads, 0, st>>>(n, sigs, digests, hlen, table, w, keys, status);
 }
 #endif
 

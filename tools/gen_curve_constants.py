@@ -106,7 +106,19 @@ def words(x, n):
     return ", ".join("0x%08xu" % ((x >> (32 * i)) & 0xffffffff) for i in range(n))
 
 
-def field_block(tag, mod, n):
+def tonelli_shanks_params(p):
+    """(s, Q, z) with p - 1 = Q * 2^s, Q odd, and z the smallest non-residue counting up from 0: the choices of the
+    reference's fp_sqrt (src/fp/fp_sqrt.c:167-199)."""
+    s, Q = 0, p - 1
+    while Q % 2 == 0:
+        s, Q = s + 1, Q // 2
+    z = 0
+    while pow(z, (p - 1) // 2, p) != p - 1:
+        z += 1
+    return s, Q, z
+
+
+def field_block(tag, mod, n, sqrt=False):
     R = 1 << (32 * n)
     m0 = (-pow(mod, -1, 1 << 32)) % (1 << 32)
     out = []
@@ -119,6 +131,14 @@ def field_block(tag, mod, n):
     out.append("    ECC_CONST_ARRAY(ONE, %d, %s);    /* R mod m */" % (n, words(R % mod, n)))
     out.append("    ECC_CONST_ARRAY(RR, %d, %s);     /* R^2 mod m */" % (n, words(R * R % mod, n)))
     out.append("    ECC_CONST_ARRAY(PM2, %d, %s);    /* m - 2 (Fermat exponent) */" % (n, words(mod - 2, n)))
+    if sqrt:
+        # Tonelli-Shanks (Field::sqrt, fp.cuh): m - 1 = Q * 2^SQRT_S; used only where SQRT_S > 1
+        s, Q, z = tonelli_shanks_params(mod)
+        out.append("    static constexpr int SQRT_S = %d;  /* 2-adicity of m - 1 */" % s)
+        out.append("    ECC_CONST_ARRAY(SQRT_QH, %d, %s);  /* (Q - 1) / 2, Q the odd part of m - 1 */"
+                   % (n, words((Q - 1) // 2, n)))
+        out.append("    ECC_CONST_ARRAY(SQRT_C, %d, %s);   /* z^Q * R mod m, z = %d the smallest non-residue */"
+                   % (n, words(pow(z, Q, mod) * R % mod, n), z))
     out.append("};")
     return out
 
@@ -131,7 +151,7 @@ def main():
         a_kind = 0 if a == p - 3 else (1 if a == 0 else 2)   # selects the doubling formula in ec.cuh
         assert (gy * gy - (gx ** 3 + a * gx + b)) % p == 0
         R = 1 << (32 * n)
-        lines += field_block("Fp_%s" % name, p, n)
+        lines += field_block("Fp_%s" % name, p, n, sqrt=True)
         lines += field_block("Fq_%s" % name, q, n)
         lines.append("struct Curve_%s {" % name)
         lines.append("    typedef Fp_%s Fp;" % name)
