@@ -44,6 +44,8 @@ ABI_SYMBOLS = [
     "eccb200_schnorr_sign_msgs_batch", "eccb200_schnorr_sign_msgs_batch_dev", "eccb200_sign_msgs_batch",
     "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len", "eccb200_verify_msgs_batch", "eccb200_verify_msgs_batch_dev",
     "eccb200_ecdsa_recover_batch", "eccb200_ecdsa_recover_batch_dev",
+    "eccb200_decdsa_sign_batch", "eccb200_decdsa_sign_batch_dev", "eccb200_ecdsa_sign_msgs_batch",
+    "eccb200_ecdsa_sign_msgs_batch_dev",
 ]
 
 _lib = None
@@ -144,6 +146,11 @@ def load_library() -> ctypes.CDLL:
     lib.eccb200_ecdsa_verify_keystate_batch.argtypes = [vp, u32, u8p, u8p, i8p, u8p, u32, i8p]
     lib.eccb200_ecdsa_recover_batch.argtypes = [vp, u32, u8p, u8p, u32, u8p, i8p]
     lib.eccb200_ecdsa_recover_batch_dev.argtypes = [vp, u32, u8p, u8p, u32, u8p, i8p, vp]
+    lib.eccb200_decdsa_sign_batch.argtypes = [vp, ctypes.c_int, u32, u8p, u8p, u8p, i8p]
+    lib.eccb200_decdsa_sign_batch_dev.argtypes = [vp, ctypes.c_int, u32, u8p, u8p, u8p, i8p, vp]
+    lib.eccb200_ecdsa_sign_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, i8p]
+    lib.eccb200_ecdsa_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, i8p,
+                                                      vp]
     lib.eccb200_host_alloc.argtypes = [ctypes.c_size_t]
     lib.eccb200_host_alloc.restype = ctypes.c_void_p
     lib.eccb200_host_alloc_input.argtypes = [ctypes.c_size_t]
@@ -448,6 +455,55 @@ class Engine:
             self._h, self.SIGN_ALGS[alg], self.SIGN_HASH_IDS[hash_name], n, d_privkeys.data_ptr(), ptr(d_pubkeys),
             d_nonces.data_ptr(), d_msgs.data_ptr(), d_offsets.data_ptr(), ptr(d_ids), ptr(d_id_offsets),
             d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_sign_msgs_batch_dev")
+
+    ECDSA_ALGS = {"ECDSA": 1, "DECDSA": 14}  # libecc ec_alg_type values
+    DECDSA_HASH_IDS = dict(SIGN_HASH_IDS, SHA224=1)  # the deterministic / message ECDSA signers also take SHA-224
+    DECDSA_HASH_LEN = dict(HASH_LEN, SHA224=28, SM3=32)
+
+    def decdsa_sign_batch(self, hash_name: str, privkeys, digests) -> Tuple[np.ndarray, np.ndarray]:
+        """Deterministic ECDSA (RFC 6979 nonces derived on the device) of digests[n, digest size of hash_name].
+        Returns (sigs[n, 2*qlen], status[n]): 0 OK, -1 ERR, 2 RETRY (see include/libecc_b200.h)."""
+        hl = self.DECDSA_HASH_LEN[hash_name]
+        d = _as_u8(privkeys)
+        n = d.size // self.qlen
+        dg = _as_u8(digests, n * hl)
+        sigs = np.zeros((n, 2 * self.qlen), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_decdsa_sign_batch(self._h, self.DECDSA_HASH_IDS[hash_name], n, d.ctypes.data,
+                                                       dg.ctypes.data, sigs.ctypes.data, status.ctypes.data),
+                    "eccb200_decdsa_sign_batch")
+        return sigs, status
+
+    def decdsa_sign_batch_dev(self, hash_name: str, d_privkeys, d_digests, d_sigs, d_status, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`)."""
+        n = d_privkeys.numel() // self.qlen
+        self._check(self.lib.eccb200_decdsa_sign_batch_dev(
+            self._h, self.DECDSA_HASH_IDS[hash_name], n, d_privkeys.data_ptr(), d_digests.data_ptr(), d_sigs.data_ptr(),
+            d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_decdsa_sign_batch_dev")
+
+    def ecdsa_sign_msgs_batch(self, alg: str, hash_name: str, privkeys, msgs, nonces=None) -> Tuple[np.ndarray, np.ndarray]:
+        """ECDSA (the caller's nonces, qlen bytes each) or DECDSA (RFC 6979 nonces, `nonces` ignored) signatures of raw
+        messages, hashed on the device.  Returns (sigs[n, 2*qlen], status[n]): 0 OK, -1 ERR, 2 RETRY."""
+        n = len(msgs)
+        d = _as_u8(privkeys, n * self.qlen)
+        k = _as_u8(nonces, n * self.qlen) if nonces is not None else None
+        blob, off = self._pack_msgs(msgs)
+        sigs = np.zeros((n, 2 * self.qlen), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_ecdsa_sign_msgs_batch(
+            self._h, self.ECDSA_ALGS[alg], self.DECDSA_HASH_IDS[hash_name], n, d.ctypes.data,
+            k.ctypes.data if k is not None else None, blob.ctypes.data, off.ctypes.data, sigs.ctypes.data,
+            status.ctypes.data), "eccb200_ecdsa_sign_msgs_batch")
+        return sigs, status
+
+    def ecdsa_sign_msgs_batch_dev(self, alg: str, hash_name: str, d_privkeys, d_msgs, d_offsets, d_sigs, d_status,
+                                  d_nonces=None, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`); d_offsets: n + 1 uint64 entries, not re-checked."""
+        n = d_privkeys.numel() // self.qlen
+        self._check(self.lib.eccb200_ecdsa_sign_msgs_batch_dev(
+            self._h, self.ECDSA_ALGS[alg], self.DECDSA_HASH_IDS[hash_name], n, d_privkeys.data_ptr(),
+            d_nonces.data_ptr() if d_nonces is not None else None, d_msgs.data_ptr(), d_offsets.data_ptr(),
+            d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_ecdsa_sign_msgs_batch_dev")
 
     VERIFY_ALGS = {"ECKCDSA": 2, "ECSDSA": 3, "ECOSDSA": 4, "ECGDSA": 6, "ECRDSA": 7, "SM2": 8}  # ec_alg_type values
 

@@ -23,6 +23,7 @@
 #include "fp.cuh"
 #include "sha2.cuh"
 #include "sm3.cuh"
+#include "hmac.cuh"
 
 namespace eccb200 {
 
@@ -701,6 +702,60 @@ template <class C> ECC_HD void digest_to_scalar(Fe<C::N> &e, const uint8_t *h, u
 		}
 	}
 	scalar_reduce<C>(e);
+}
+
+/*
+ * The deterministic ECDSA nonce of RFC 6979 §3.2 as the reference derives it (__ecdsa_rfc6979_nonce,
+ * sig/ecdsa_common.c:48-169), with HMAC over hash_type (hmac.cuh) and h the hsize-byte digest H(m):
+ *   b, c. V = 0x01 .. 0x01, K = 0x00 .. 0x00 (hsize bytes each)                                          (:74-75)
+ *   d.    K = HMAC_K(V || 0x00 || int2octets(x) || bits2octets(h)), bits2octets(h) = ((h >> max(0, 8*hsize -
+ *         qbits)) mod q) on qlen bytes                                                                     (:81-97)
+ *   e-g.  V = HMAC_K(V); K = HMAC_K(V || 0x01 || x || bits2octets(h)); V = HMAC_K(V)                     (:100-116)
+ *   h.    T = the V = HMAC_K(V) blocks until T has qbits bits, k = leftmost qbits bits of T; while k >= q,
+ *         K = HMAC_K(V || 0x00), V = HMAC_K(V), and again                                                (:136-165)
+ * x must be in [1, q-1].  The reference takes a k of 0 (it checks k >= q only); the signer reports that k as
+ * ECCB200_ERR.  V || b || x || bits2octets(h) is the two-segment source: V, then b || x || bits2octets(h) in one
+ * thread-held buffer.  Returns the number of k >= q retries (the host tests count them).
+ */
+template <class C>
+ECC_D int rfc6979_nonce(Fe<C::N> &k, int hash_type, const Fe<C::N> &x, const uint8_t *h, uint32_t hsize)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, QL = C::QLEN, SH = 8 * C::QLEN - C::QBITS;
+	uint8_t V[64], K[64], bxh[1 + 2 * QL], T[QL];
+	for (uint32_t i = 0; i < hsize; i++) {
+		V[i] = 0x01;
+		K[i] = 0x00;
+	}
+	Fe<N> h1;
+	digest_to_scalar<C>(h1, h, hsize); /* leftmost min(8*hsize, qbits) bits, mod q */
+	bxh[0] = 0x00;
+	store_be<N>(bxh + 1, x, QL);
+	store_be<N>(bxh + 1 + QL, h1, QL);
+	const uint64_t mlen = (uint64_t)hsize + 1 + 2 * QL;
+	hmac_src(hash_type, K, hsize, Seg2{ V, hsize, bxh }, mlen, K);         /* d */
+	hmac_src(hash_type, K, hsize, ByteSpan{ V }, hsize, V);                 /* e */
+	bxh[0] = 0x01;
+	hmac_src(hash_type, K, hsize, Seg2{ V, hsize, bxh }, mlen, K);         /* f */
+	hmac_src(hash_type, K, hsize, ByteSpan{ V }, hsize, V);                 /* g */
+	const uint8_t zero = 0x00;
+	for (int retries = 0;; retries++) {
+		for (int t = 0; t < QL; t += (int)hsize) {                      /* h.2 */
+			hmac_src(hash_type, K, hsize, ByteSpan{ V }, hsize, V);
+			for (int i = 0; i < (int)hsize && t + i < QL; i++) T[t + i] = V[i];
+		}
+		load_be<N>(k, T, QL);                                          /* h.3: bits2int(T) */
+		if (SH > 0) {
+#pragma unroll
+			for (int j = 0; j < N; j++) {
+				const uint32_t hi = (j + 1 < N) ? k.w[j + 1] : 0u;
+				k.w[j] = (k.w[j] >> SH) | (hi << ((32 - SH) & 31));
+			}
+		}
+		if (!Fq::geq_mod(k)) return retries;
+		hmac_src(hash_type, K, hsize, Seg2{ V, hsize, &zero }, (uint64_t)hsize + 1, K);
+		hmac_src(hash_type, K, hsize, ByteSpan{ V }, hsize, V);
+	}
 }
 
 /* u = e * s^-1 mod q, v = r * s^-1 mod q (plain form): the mod-q scalar preparation of __ecdsa_verify_finalize

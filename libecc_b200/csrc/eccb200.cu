@@ -87,8 +87,9 @@ struct eccb200_ctx {
 	uint8_t *unique_io = nullptr; /* device buffer of eccb200_prj_pt_unique_batch (in || out || status), grown on demand:
 	                               * a cudaMalloc / cudaFree pair per call cost up to a second on a busy allocator */
 	size_t unique_io_bytes = 0;
-	uint8_t *sign_k = nullptr; /* [sign_k_cap][qlen] BIP0340 nonces of the device-pointer Schnorr signer, grown on demand */
-	uint32_t sign_k_cap = 0;
+	uint8_t *sign_k = nullptr; /* [sign_k_cap][qlen] scratch of the device-pointer signers, grown on demand: BIP0340 and
+	                            * RFC 6979 nonces, and the digests of the ECDSA message signer after them */
+	size_t sign_k_cap = 0;
 	/* optional per-kernel timing of the device-pointer API (bench.py's roofline leg) */
 	bool profiling = false;
 	static const int kProfCalls = 64;
@@ -1694,6 +1695,19 @@ static int schnorr_sign_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint3
 	});
 }
 
+/* ctx->sign_k holds at least `slots` qlen-byte entries */
+static int ensure_sign_k(eccb200_ctx *ctx, size_t slots)
+{
+	if (ctx->sign_k_cap >= slots) return 0;
+	CUDA_OK(cudaDeviceSynchronize()); /* an earlier call may still read the buffer that is about to be replaced */
+	if (ctx->sign_k) cudaFree(ctx->sign_k);
+	ctx->sign_k = nullptr;
+	ctx->sign_k_cap = 0;
+	CUDA_OK(cudaMalloc(&ctx->sign_k, slots * ctx->qlen));
+	ctx->sign_k_cap = slots;
+	return 0;
+}
+
 extern "C" int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
 						   const uint8_t *d_privkeys, const uint8_t *d_pubkeys,
 						   const uint8_t *d_randomness, const uint8_t *d_msgs,
@@ -1709,14 +1723,7 @@ extern "C" int eccb200_schnorr_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_typ
 	if (n == 0) return 0;
 	CUDA_OK(cudaSetDevice(ctx->device));
 	if (ensure_work(ctx, n)) return -1;
-	if (sig_type == SIG_BIP0340 && ctx->sign_k_cap < n) {
-		CUDA_OK(cudaDeviceSynchronize()); /* an earlier call may still read the buffer that is about to be replaced */
-		if (ctx->sign_k) cudaFree(ctx->sign_k);
-		ctx->sign_k = nullptr;
-		ctx->sign_k_cap = 0;
-		CUDA_OK(cudaMalloc(&ctx->sign_k, (size_t)n * ctx->qlen));
-		ctx->sign_k_cap = n;
-	}
+	if (sig_type == SIG_BIP0340 && ensure_sign_k(ctx, n)) return -1;
 	return schnorr_sign_dev(ctx, sig_type, hash_type, n, d_privkeys, d_pubkeys, d_randomness, d_msgs, d_offsets, d_sigs,
 				d_status, ctx->jac, ctx->prefix, ctx->aff, ctx->sign_k, (cudaStream_t)stream);
 }
@@ -1963,6 +1970,128 @@ extern "C" int eccb200_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_
 							       ch.rag_base[0], ch.rag_off[0], ch.rag_base[1], ch.rag_off[1],
 							       ch.sigs, ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
 							       ctx->stage_aff[s], ctx->streams[s]);
+				  });
+}
+
+/* ------------------------------------------------------- deterministic ECDSA (RFC 6979) and ECDSA of raw messages */
+
+enum { SIG_ECDSA = 1, SIG_DECDSA = 14 }; /* ec_alg_type values of the reference (lib_ecc_types.h) */
+static const char *kDecdsaHashMsg =
+	"unsupported hash (SHA224 = 1, SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224..512 = 5..8, SM3 = 11)";
+
+/* The nonce kernel (H(m) into dig_buf when msgs are given, the RFC 6979 k into k_buf when det), K1 on k (k_buf, or
+ * the caller's d_nonce), K4, k_ecdsa_sign_finish on the digests (dig_buf, or the caller's d_dig) — all on `st`. */
+static int ecdsa_det_sign_dev(eccb200_ctx *ctx, bool det, int hash_type, uint32_t n, const uint8_t *d_priv,
+			      const uint8_t *d_nonce, const uint8_t *d_dig, bool with_msgs, const uint8_t *d_msgs,
+			      const uint64_t *d_off, uint8_t *k_buf, uint8_t *dig_buf, uint8_t *d_sigs, int8_t *d_status,
+			      uint32_t *jac, uint32_t *prefix, uint8_t *aff, cudaStream_t st)
+{
+	if (n == 0) return 0;
+	const uint32_t ds = (uint32_t)decdsa_hash_digest_size(hash_type);
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		const uint8_t *k = det ? k_buf : d_nonce, *dig = with_msgs ? dig_buf : d_dig;
+		LaunchMisc<C>::ecdsa_nonce(n, hash_type, d_priv, d_dig, d_msgs, d_off, with_msgs ? dig_buf : nullptr,
+					   det ? k_buf : nullptr, st);                       /* H(m), k      */
+		LaunchFixed<C>::fixed(n, k, ctx->table, ctx->w, jac, d_status, st);             /* k*G          */
+		LaunchMisc<C>::to_affine(affine_grid(ctx, n), n, jac, prefix, aff, d_status, st); /* affine (x, y) */
+		LaunchMisc<C>::sign_finish(affine_grid(ctx, n), n, d_priv, k, dig, ds, aff, prefix, d_sigs, d_status,
+					   st);                                                   /* r, s         */
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 4;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+extern "C" int eccb200_decdsa_sign_batch_dev(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *d_privkeys,
+					     const uint8_t *d_digests, uint8_t *d_sigs, int8_t *d_status, void *stream)
+{
+	if (!ctx) return fail("null argument");
+	if (!decdsa_hash_digest_size(hash_type)) return fail(kDecdsaHashMsg);
+	if (n && (!d_privkeys || !d_digests || !d_sigs || !d_status)) return fail("null argument");
+	if (misaligned16(ctx, { d_privkeys, d_sigs })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	if (ensure_work(ctx, n) || ensure_sign_k(ctx, n)) return -1;
+	return ecdsa_det_sign_dev(ctx, true, hash_type, n, d_privkeys, nullptr, d_digests, false, nullptr, nullptr,
+				  ctx->sign_k, nullptr, d_sigs, d_status, ctx->jac, ctx->prefix, ctx->aff,
+				  (cudaStream_t)stream);
+}
+
+/* Host-pointer form through sign_msgs_pipeline: private keys and digests as columns, k in the scratch column. */
+extern "C" int eccb200_decdsa_sign_batch(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *privkeys,
+					 const uint8_t *digests, uint8_t *sigs, int8_t *status)
+{
+	if (!ctx) return fail("null argument");
+	const int ds = decdsa_hash_digest_size(hash_type);
+	if (!ds) return fail(kDecdsaHashMsg);
+	if (n && (!privkeys || !digests || !sigs || !status)) return fail("null argument");
+	if (n == 0) return 0;
+	const size_t ql = ctx->qlen;
+	const SignCol cols[3] = { { privkeys, ql }, { digests, (size_t)ds }, { nullptr, 0 } };
+	const SignRagged rag[2] = { { nullptr, nullptr }, { nullptr, nullptr } };
+	return sign_msgs_pipeline(ctx, n, cols, ql, rag, 2 * ql, sigs, status,
+				  [&](int s, uint32_t cnt, const SignChunk &ch) {
+					  return ecdsa_det_sign_dev(ctx, true, hash_type, cnt, ch.col[0], nullptr, ch.col[1],
+								    false, nullptr, nullptr, ch.scratch, nullptr, ch.sigs,
+								    ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
+								    ctx->stage_aff[s], ctx->streams[s]);
+				  });
+}
+
+/* the checks both message forms share; 0, or -1 with the reason in eccb200_last_error */
+static int ecdsa_msgs_args(const eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const void *privkeys,
+			   const void *nonces, const void *offsets, const void *sigs, const void *status)
+{
+	if (!ctx) return fail("null argument");
+	if (sig_type != SIG_ECDSA && sig_type != SIG_DECDSA) return fail("unsupported sig_type (ECDSA = 1, DECDSA = 14)");
+	if (!decdsa_hash_digest_size(hash_type)) return fail(kDecdsaHashMsg);
+	if (sig_type == SIG_ECDSA && !nonces) return fail("ECDSA needs the caller's nonces");
+	if (n && (!privkeys || !offsets || !sigs || !status)) return fail("null argument");
+	return 0;
+}
+
+/* Scratch of the message forms, per chunk of cnt items: the RFC 6979 nonces (DECDSA, cnt * qlen bytes), then the
+ * digests (cnt * digest size bytes).  cnt * qlen keeps the digests 16-byte aligned wherever alignment matters. */
+extern "C" int eccb200_ecdsa_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+						 const uint8_t *d_privkeys, const uint8_t *d_nonces, const uint8_t *d_msgs,
+						 const uint64_t *d_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream)
+{
+	if (ecdsa_msgs_args(ctx, sig_type, hash_type, n, d_privkeys, d_nonces, d_offsets, d_sigs, d_status)) return -1;
+	const bool det = sig_type == SIG_DECDSA;
+	if (misaligned16(ctx, { d_privkeys, det ? nullptr : d_nonces, d_sigs })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	const size_t ql = ctx->qlen, ds = (size_t)decdsa_hash_digest_size(hash_type);
+	const size_t k_bytes = det ? (size_t)n * ql : 0;
+	if (ensure_work(ctx, n) || ensure_sign_k(ctx, (k_bytes + (size_t)n * ds + ql - 1) / ql)) return -1;
+	return ecdsa_det_sign_dev(ctx, det, hash_type, n, d_privkeys, det ? nullptr : d_nonces, nullptr, true, d_msgs,
+				  d_offsets, det ? ctx->sign_k : nullptr, ctx->sign_k + k_bytes, d_sigs, d_status, ctx->jac,
+				  ctx->prefix, ctx->aff, (cudaStream_t)stream);
+}
+
+extern "C" int eccb200_ecdsa_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					     const uint8_t *privkeys, const uint8_t *nonces, const uint8_t *msgs,
+					     const uint64_t *offsets, uint8_t *sigs, int8_t *status)
+{
+	if (ecdsa_msgs_args(ctx, sig_type, hash_type, n, privkeys, nonces, offsets, sigs, status)) return -1;
+	if (n == 0) return 0;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	const bool det = sig_type == SIG_DECDSA;
+	const size_t ql = ctx->qlen, ds = (size_t)decdsa_hash_digest_size(hash_type);
+	const SignCol cols[3] = { { privkeys, ql }, { det ? nullptr : nonces, ql }, { nullptr, 0 } };
+	const SignRagged rag[2] = { { msgs, offsets }, { nullptr, nullptr } };
+	return sign_msgs_pipeline(ctx, n, cols, (det ? ql : 0) + ds, rag, 2 * ql, sigs, status,
+				  [&](int s, uint32_t cnt, const SignChunk &ch) {
+					  const size_t k_bytes = det ? (size_t)cnt * ql : 0;
+					  return ecdsa_det_sign_dev(ctx, det, hash_type, cnt, ch.col[0], ch.col[1], nullptr,
+								    true, ch.rag_base[0], ch.rag_off[0],
+								    det ? ch.scratch : nullptr, ch.scratch + k_bytes,
+								    ch.sigs, ch.status, ctx->stage_jac[s],
+								    ctx->stage_prefix[s], ctx->stage_aff[s], ctx->streams[s]);
 				  });
 }
 

@@ -1154,6 +1154,37 @@ __global__ void __launch_bounds__(128) k_ecdsa_sign_finish(uint32_t n, const uin
 	}
 }
 
+/*
+ * Before K1 of the deterministic and raw-message forms of the ECDSA signer, one item per thread.  With dig_out: the
+ * digest H(m) into dig_out ([n][digest size]; message i is msgs[off[i] .. off[i+1]), as k_sha2_batch).  With k_out: the
+ * RFC 6979 nonce of x and that digest (or of digests[i] without dig_out) into k_out (rfc6979_nonce), or 0 without any
+ * HMAC work where x is outside [1, q-1] (k_ecdsa_sign_finish then reports ECCB200_ERR).  hash_type: 1..8 or 11.
+ */
+template <class C>
+__global__ void __launch_bounds__(128) k_ecdsa_nonce(uint32_t n, int hash_type, const uint8_t *__restrict__ privkeys,
+						     const uint8_t *__restrict__ digests, const uint8_t *__restrict__ msgs,
+						     const uint64_t *__restrict__ off, uint8_t *__restrict__ dig_out,
+						     uint8_t *__restrict__ k_out)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N;
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	const uint32_t ds = (uint32_t)decdsa_hash_digest_size(hash_type);
+	uint8_t hm[64];
+	const uint8_t *h = dig_out ? hm : digests + (size_t)idx * ds;
+	if (dig_out) {
+		decdsa_hash_src(hash_type, ByteSpan{ msgs + off[idx] }, off[idx + 1] - off[idx], hm);
+		for (uint32_t i = 0; i < ds; i++) dig_out[(size_t)idx * ds + i] = hm[i];
+	}
+	if (!k_out) return;
+	Fe<N> x, k;
+	load_wire<N, C::QLEN>(x, privkeys + (size_t)idx * C::QLEN);
+	Fq::set_zero(k);
+	if (!Fq::is_zero(x) && !Fq::geq_mod(x)) rfc6979_nonce<C>(k, hash_type, x, h, ds);
+	store_wire<N, C::QLEN>(k_out + (size_t)idx * C::QLEN, k);
+}
+
 /* ------------------------------------------------------------------------- ECKCDSA / ECGDSA / ECRDSA / SM2 sign */
 
 /*
@@ -1633,6 +1664,8 @@ template <class C> struct LaunchMisc {
 	static void sign_finish(uint32_t blocks, uint32_t n, const uint8_t *privkeys, const uint8_t *nonces,
 				const uint8_t *digests, uint32_t hlen, const uint8_t *kG_aff, uint32_t *prefix,
 				uint8_t *sigs, int8_t *status, cudaStream_t st);
+	static void ecdsa_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *digests,
+				const uint8_t *msgs, const uint64_t *off, uint8_t *dig_out, uint8_t *k_out, cudaStream_t st);
 	static void bip0340_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *pubkeys,
 				  const uint8_t *aux, const uint8_t *msgs, const uint64_t *off, uint8_t *k_out,
 				  cudaStream_t st);
@@ -1739,6 +1772,12 @@ void LaunchMisc<C>::sign_finish(uint32_t blocks, uint32_t n, const uint8_t *priv
 {
 	k_ecdsa_sign_finish<C><<<blocks, kThreads, 0, st>>>(n, privkeys, nonces, digests, hlen, kG_aff, prefix, sigs,
 							     status);
+}
+template <class C>
+void LaunchMisc<C>::ecdsa_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *digests,
+				const uint8_t *msgs, const uint64_t *off, uint8_t *dig_out, uint8_t *k_out, cudaStream_t st)
+{
+	k_ecdsa_nonce<C><<<grid_for(n), kThreads, 0, st>>>(n, hash_type, privkeys, digests, msgs, off, dig_out, k_out);
 }
 template <class C>
 void LaunchMisc<C>::bip0340_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *pubkeys,

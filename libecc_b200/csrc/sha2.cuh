@@ -1,6 +1,7 @@
 /*
  * sha2.cuh — SHA-256 / SHA-384 / SHA-512 of short messages on the device (SURVEY.md §8f.3: "host-side hashing on
- * device", the step before the ECDSA path).  One thread hashes one message of arbitrary length.
+ * device", the step before the ECDSA path), and SHA-224 for the deterministic ECDSA signer (hmac.cuh).  One thread
+ * hashes one message of arbitrary length.
  *
  * Reference counterparts (relative to /root/reference/src): sha256_init/update/final hash/sha256.c:70,96,145 (scattered
  * form :201), SHA-384/512 hash/sha384.c, hash/sha512.c over hash/sha512_core.c; generic front end hash_mapping
@@ -51,12 +52,20 @@ template <class Src> SHA2_D uint32_t padded_byte(const Src &m, uint64_t len, uin
 	return (i < len) ? m[i] : ((i == len) ? 0x80u : 0u);
 }
 
-/* digest: 32 bytes, big-endian words */
-template <class Src> SHA2_D void sha256_src(const Src &m, uint64_t len, uint8_t *__restrict__ digest)
+/* SHA-224's initial value (FIPS 180-4 §5.3.2) */
+SHA2_D uint32_t sha224_iv(int i)
+{
+	return i == 0 ? 0xc1059ed8u : i == 1 ? 0x367cd507u : i == 2 ? 0x3070dd17u : i == 3 ? 0xf70e5939u :
+	       i == 4 ? 0xffc00b31u : i == 5 ? 0x68581511u : i == 6 ? 0x64f98fa7u : 0xbefa4fa4u;
+}
+
+/* digest: 32 bytes, big-endian words; sha224: SHA-224 (the same compression from its own initial value, 28 bytes out) */
+template <class Src>
+SHA2_D void sha256_src(const Src &m, uint64_t len, uint8_t *__restrict__ digest, bool sha224 = false)
 {
 	uint32_t h[8];
 #pragma unroll
-	for (int i = 0; i < 8; i++) h[i] = kSha256H[i];
+	for (int i = 0; i < 8; i++) h[i] = sha224 ? sha224_iv(i) : kSha256H[i];
 	const uint64_t nblocks = (len + 9 + 63) / 64;
 #pragma unroll 1
 	for (uint64_t b = 0; b < nblocks; b++) {
@@ -95,6 +104,7 @@ template <class Src> SHA2_D void sha256_src(const Src &m, uint64_t len, uint8_t 
 	}
 #pragma unroll
 	for (int i = 0; i < 8; i++) {
+		if (sha224 && i == 7) break;
 		digest[4 * i] = (uint8_t)(h[i] >> 24);
 		digest[4 * i + 1] = (uint8_t)(h[i] >> 16);
 		digest[4 * i + 2] = (uint8_t)(h[i] >> 8);
