@@ -267,6 +267,64 @@ int eccb200_ecdsa_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_t
 				      const uint64_t *d_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream);
 
 /*
+ * BIGN (sig_type ECCB200_ALG_BIGN, the caller's nonces) or DBIGN (ECCB200_ALG_DBIGN, deterministic nonces; nonces
+ * ignored, may be NULL) signatures of raw messages, hashed on the device: ec_sign(…, BIGN | DBIGN, hash_type, adata,
+ * adata_len) per item (__bign_sign_finalize, src/sig/bign_common.c:468-722), with l = qlen / 2:
+ *   H = hash(m); W = k*G affine; s0 = the first min(l, 32) bytes of BELT-HASH(oid || the first 2l bytes of LE(W_x) ||
+ *   H), zero-padded to l bytes (on SECP521R1, l = 33 and s0[32] = 0); s1 = (k - h - (s0 + 2^(8l)) * x) mod q with
+ *   h = OS2I(reverse(H)) mod q and s0 read little-endian.  There is no restart case: s1 = 0 is emitted.
+ * DBIGN derives k as __bign_determinitic_nonce (:200-342) does: belt-block rounds keyed by BELT-HASH(oid || the first
+ * 2l bytes of LE(x) || t) over H zero-padded to n = max(2, hlen / 16) blocks, at least 2n rounds, until 0 < k < q.
+ *   privkeys, nonces : n * qlen bytes each (nonces: BIGN only), big-endian, values in [1, q-1] (else ECCB200_ERR)
+ *   msgs / offsets   : message i is msgs[offsets[i] .. offsets[i+1]), offsets has n + 1 entries
+ *   adata / adata_offsets : item i's record adata[adata_offsets[i] .. adata_offsets[i+1]), the reference's layout
+ *                (bign_set_adata, :149-183): oid_len (2 bytes, big-endian) || t_len (2 bytes, big-endian) || oid || t,
+ *                trailing bytes allowed.  Empty, shorter than 4 bytes, oid_len + t_len > len - 4 or longer than 65535
+ *                bytes (the reference's adata_len is a u16; :97-147) is ECCB200_ERR.  The OID is not checked against
+ *                the hash; t is used by DBIGN only.
+ *   hash_type        : 1 (SHA224), 2 .. 8 (SHA256 .. SHA3_512), 11 (SM3), 16 (BELT_HASH) or 17 .. 20 (BASH224 ..
+ *                BASH512).  16 .. 20 are accepted by the four BIGN entry points only.
+ *   sigs             : n * (l + qlen) bytes s0 || LE(s1) (36, 42, 48, 72, 96 or 99 bytes per item), zero unless OK
+ *   status           : ECCB200_OK or ECCB200_ERR (x or the BIGN nonce outside [1, q-1], or a malformed record)
+ * An unsupported sig_type or hash_type, BIGN without nonces, a NULL buffer, or (host form) offsets or adata_offsets
+ * that do not start at 0 or that decrease return -1 (eccb200_last_error) and write nothing; n = 0 returns 0.  The
+ * _dev form keeps its scratch (k, digests) in the context, grown on demand, does not re-check the offsets, and needs
+ * 16-byte alignment of the privkey, nonce and signature buffers on the 256/384/512-bit curves, not of d_msgs or
+ * d_adata.
+ * NOTE: like every entry point of this library this is a throughput path, NOT a constant-time one.
+ */
+#define ECCB200_ALG_BIGN 18
+#define ECCB200_ALG_DBIGN 19
+#define ECCB200_HASH_BELT_HASH 16
+int eccb200_bign_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const uint8_t *privkeys,
+				 const uint8_t *nonces, const uint8_t *msgs, const uint64_t *offsets, const uint8_t *adata,
+				 const uint64_t *adata_offsets, uint8_t *sigs, int8_t *status);
+int eccb200_bign_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+				     const uint8_t *d_privkeys, const uint8_t *d_nonces, const uint8_t *d_msgs,
+				     const uint64_t *d_offsets, const uint8_t *d_adata, const uint64_t *d_adata_offsets,
+				     uint8_t *d_sigs, int8_t *d_status, void *stream);
+
+/*
+ * BIGN / DBIGN verification of raw messages (both schemes verify alike): ec_verify(…, BIGN, hash_type, adata,
+ * adata_len) per item (__bign_verify_init / __bign_verify_finalize, src/sig/bign_common.c:742-993).  Reject s1 >= q;
+ * W' = ((s1 + h) mod q)*G + (s0 + 2^(8l))*Y; reject W' at infinity; accept iff s0 equals the first l bytes of
+ * BELT-HASH(oid || the first 2l bytes of LE(W'_x) || H), zero-padded as in signing.  One kernel checks the record and
+ * s1, hashes the message and prepares the scalars, the double-scalar kernel of eccb200_verify_msgs_batch computes W',
+ * and one kernel runs the BELT-HASH test.
+ *   sigs : n * (l + qlen) bytes;  pubkeys : n * 2*plen affine keys;  msgs, adata, hash_type : as the signer
+ *   verdict : 0 valid, -1 invalid (a malformed record, s1 >= q, a key off the curve, or a failed test)
+ * Argument errors as the signer.  The _dev form: 16-byte alignment of the signature and key buffers on the
+ * 256/384/512-bit curves.
+ */
+int eccb200_bign_verify_msgs_batch(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *sigs,
+				   const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *offsets,
+				   const uint8_t *adata, const uint64_t *adata_offsets, int8_t *verdict);
+int eccb200_bign_verify_msgs_batch_dev(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *d_sigs,
+				       const uint8_t *d_pubkeys, const uint8_t *d_msgs, const uint64_t *d_offsets,
+				       const uint8_t *d_adata, const uint64_t *d_adata_offsets, int8_t *d_verdict,
+				       void *stream);
+
+/*
  * Batched ECC-CDH shared-secret derivation: ecccdh_derive_secret (src/ecdh/ecccdh.c:167-233) per item — peer key
  * import with on-curve check (src/sig/ec_key.c:181-214), prj_pt_mul(d, Q) (:209), reject infinity (:216-217),
  * export of the affine x coordinate (:220-224).

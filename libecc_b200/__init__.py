@@ -45,7 +45,8 @@ ABI_SYMBOLS = [
     "eccb200_sign_msgs_batch_dev", "eccb200_sign_sig_len", "eccb200_verify_msgs_batch", "eccb200_verify_msgs_batch_dev",
     "eccb200_ecdsa_recover_batch", "eccb200_ecdsa_recover_batch_dev",
     "eccb200_decdsa_sign_batch", "eccb200_decdsa_sign_batch_dev", "eccb200_ecdsa_sign_msgs_batch",
-    "eccb200_ecdsa_sign_msgs_batch_dev",
+    "eccb200_ecdsa_sign_msgs_batch_dev", "eccb200_bign_sign_msgs_batch", "eccb200_bign_sign_msgs_batch_dev",
+    "eccb200_bign_verify_msgs_batch", "eccb200_bign_verify_msgs_batch_dev",
 ]
 
 _lib = None
@@ -151,6 +152,12 @@ def load_library() -> ctypes.CDLL:
     lib.eccb200_ecdsa_sign_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, i8p]
     lib.eccb200_ecdsa_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, i8p,
                                                       vp]
+    lib.eccb200_bign_sign_msgs_batch.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp, u8p,
+                                                 i8p]
+    lib.eccb200_bign_sign_msgs_batch_dev.argtypes = [vp, ctypes.c_int, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp,
+                                                     u8p, i8p, vp]
+    lib.eccb200_bign_verify_msgs_batch.argtypes = [vp, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp, i8p]
+    lib.eccb200_bign_verify_msgs_batch_dev.argtypes = [vp, ctypes.c_int, u32, u8p, u8p, u8p, vp, u8p, vp, i8p, vp]
     lib.eccb200_host_alloc.argtypes = [ctypes.c_size_t]
     lib.eccb200_host_alloc.restype = ctypes.c_void_p
     lib.eccb200_host_alloc_input.argtypes = [ctypes.c_size_t]
@@ -179,6 +186,14 @@ def _as_u8(a, nbytes: Optional[int] = None) -> np.ndarray:
     if nbytes is not None and arr.size != nbytes:
         raise ValueError(f"expected {nbytes} bytes, got {arr.size}")
     return arr
+
+
+def bign_adata(oid: bytes, t: bytes = b"") -> bytes:
+    """The BIGN / DBIGN adata record of the reference (bign_set_adata): oid_len and t_len as 2-byte big-endian
+    integers, then the hash OID (DER content bytes), then t (DBIGN's additional nonce data)."""
+    if len(oid) + len(t) + 4 > 0xFFFF:
+        raise ValueError("BIGN adata longer than 65535 bytes")
+    return len(oid).to_bytes(2, "big") + len(t).to_bytes(2, "big") + bytes(oid) + bytes(t)
 
 
 def pinned_empty(shape, dtype=np.uint8, write_combined: bool = False) -> np.ndarray:
@@ -504,6 +519,67 @@ class Engine:
             self._h, self.ECDSA_ALGS[alg], self.DECDSA_HASH_IDS[hash_name], n, d_privkeys.data_ptr(),
             d_nonces.data_ptr() if d_nonces is not None else None, d_msgs.data_ptr(), d_offsets.data_ptr(),
             d_sigs.data_ptr(), d_status.data_ptr(), ctypes.c_void_p(stream_handle)), "eccb200_ecdsa_sign_msgs_batch_dev")
+
+    BIGN_ALGS = {"BIGN": 18, "DBIGN": 19}  # libecc ec_alg_type values
+    # the BIGN signers and verifier also take BELT-HASH and BASH (hash_alg_type 16..20)
+    BIGN_HASH_IDS = dict(DECDSA_HASH_IDS, BELT_HASH=16, BASH224=17, BASH256=18, BASH384=19, BASH512=20)
+    BIGN_HASH_LEN = dict(DECDSA_HASH_LEN, BELT_HASH=32, BASH224=28, BASH256=32, BASH384=48, BASH512=64)
+
+    @property
+    def bign_sig_len(self) -> int:
+        """Bytes of a BIGN / DBIGN signature s0 || s1: qlen / 2 + qlen."""
+        return self.qlen // 2 + self.qlen
+
+    def bign_sign_msgs_batch(self, alg: str, hash_name: str, privkeys, msgs, adata,
+                             nonces=None) -> Tuple[np.ndarray, np.ndarray]:
+        """BIGN (the caller's nonces, qlen bytes each) or DBIGN (deterministic nonces, `nonces` ignored) signatures of
+        raw messages, hashed on the device; adata[i] is item i's record (bign_adata).  Returns (sigs[n, bign_sig_len],
+        status[n]): 0 OK, -1 ERR (see include/libecc_b200.h)."""
+        n = len(msgs)
+        d = _as_u8(privkeys, n * self.qlen)
+        k = _as_u8(nonces, n * self.qlen) if nonces is not None else None
+        blob, off = self._pack_msgs(msgs)
+        ad_blob, ad_off = self._pack_msgs(adata)
+        sigs = np.zeros((n, self.bign_sig_len), dtype=np.uint8)
+        status = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_bign_sign_msgs_batch(
+            self._h, self.BIGN_ALGS[alg], self.BIGN_HASH_IDS[hash_name], n, d.ctypes.data,
+            k.ctypes.data if k is not None else None, blob.ctypes.data, off.ctypes.data, ad_blob.ctypes.data,
+            ad_off.ctypes.data, sigs.ctypes.data, status.ctypes.data), "eccb200_bign_sign_msgs_batch")
+        return sigs, status
+
+    def bign_sign_msgs_batch_dev(self, alg: str, hash_name: str, d_privkeys, d_msgs, d_offsets, d_adata,
+                                 d_adata_offsets, d_sigs, d_status, d_nonces=None, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`); offsets: n + 1 uint64 entries, not re-checked."""
+        n = d_privkeys.numel() // self.qlen
+        self._check(self.lib.eccb200_bign_sign_msgs_batch_dev(
+            self._h, self.BIGN_ALGS[alg], self.BIGN_HASH_IDS[hash_name], n, d_privkeys.data_ptr(),
+            d_nonces.data_ptr() if d_nonces is not None else None, d_msgs.data_ptr(), d_offsets.data_ptr(),
+            d_adata.data_ptr(), d_adata_offsets.data_ptr(), d_sigs.data_ptr(), d_status.data_ptr(),
+            ctypes.c_void_p(stream_handle)), "eccb200_bign_sign_msgs_batch_dev")
+
+    def bign_verify_msgs_batch(self, hash_name: str, sigs, pubkeys, msgs, adata) -> np.ndarray:
+        """BIGN / DBIGN verification of raw messages: verdict[n], 0 valid, -1 invalid."""
+        n = len(msgs)
+        sg = _as_u8(sigs, n * self.bign_sig_len)
+        pk = _as_u8(pubkeys, n * 2 * self.plen)
+        blob, off = self._pack_msgs(msgs)
+        ad_blob, ad_off = self._pack_msgs(adata)
+        verdict = np.zeros(n, dtype=np.int8)
+        self._check(self.lib.eccb200_bign_verify_msgs_batch(
+            self._h, self.BIGN_HASH_IDS[hash_name], n, sg.ctypes.data, pk.ctypes.data, blob.ctypes.data,
+            off.ctypes.data, ad_blob.ctypes.data, ad_off.ctypes.data, verdict.ctypes.data),
+            "eccb200_bign_verify_msgs_batch")
+        return verdict
+
+    def bign_verify_msgs_batch_dev(self, hash_name: str, d_sigs, d_pubkeys, d_msgs, d_offsets, d_adata,
+                                   d_adata_offsets, d_verdict, stream_handle: int = 0):
+        """Device-tensor form (asynchronous on `stream_handle`)."""
+        n = d_verdict.numel()
+        self._check(self.lib.eccb200_bign_verify_msgs_batch_dev(
+            self._h, self.BIGN_HASH_IDS[hash_name], n, d_sigs.data_ptr(), d_pubkeys.data_ptr(), d_msgs.data_ptr(),
+            d_offsets.data_ptr(), d_adata.data_ptr(), d_adata_offsets.data_ptr(), d_verdict.data_ptr(),
+            ctypes.c_void_p(stream_handle)), "eccb200_bign_verify_msgs_batch_dev")
 
     VERIFY_ALGS = {"ECKCDSA": 2, "ECSDSA": 3, "ECOSDSA": 4, "ECGDSA": 6, "ECRDSA": 7, "SM2": 8}  # ec_alg_type values
 

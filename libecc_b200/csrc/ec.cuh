@@ -24,6 +24,8 @@
 #include "sha2.cuh"
 #include "sm3.cuh"
 #include "hmac.cuh"
+#include "belt.cuh"
+#include "bash.cuh"
 
 namespace eccb200 {
 
@@ -1473,6 +1475,226 @@ ECC_D bool msgs_verify_accept(int sig_type, int hash_type, const uint8_t *sig, c
 		Fq::add(x, x, e);
 	}
 	return Fq::eq(x, r);
+}
+
+/* ----------------------------------------------------------------------- BIGN / DBIGN (STB 34.101.45) of messages */
+
+enum { SIG_BIGN = 18, SIG_DBIGN = 19 }; /* ec_alg_type values of the reference (lib_ecc_types.h) */
+constexpr uint32_t kBignMaxAdata = 0xffff; /* the reference's adata_len is a u16 */
+
+/* Digest size of the BIGN message hashes: SHA-224 (1), SHA-256 .. SHA3-512 (2..8), SM3 (11), BELT-HASH (16) and
+ * BASH224 .. BASH512 (17..20); 0 for any other type.  Only the BIGN entry points accept 16..20. */
+SHA3_HD int bign_hash_digest_size(int hash_type)
+{
+	return hash_type == HASH_BELT ? 32 : bash_digest_size(hash_type) ? bash_digest_size(hash_type) :
+									    decdsa_hash_digest_size(hash_type);
+}
+
+/* Any of them over a byte source; H is the BELT S-box (belt.cuh: shared memory on the device) */
+template <class Src>
+ECC_D void bign_hash_src(int hash_type, const Src &m, uint64_t len, uint8_t *digest, const uint8_t *H)
+{
+	if (hash_type == HASH_BELT) belt_hash_src(m, len, digest, H);
+	else if (bash_digest_size(hash_type)) bash_src(m, len, digest, bash_digest_size(hash_type));
+	else decdsa_hash_src(hash_type, m, len, digest);
+}
+
+/* The adata record oid_len (2 bytes, big-endian) || t_len (2 bytes, big-endian) || oid || t || any trailing bytes
+ * (bign_get_oid_from_adata / bign_get_t_from_adata, sig/bign_common.c:97-147): valid iff 4 <= len <= 65535 and
+ * oid_len + t_len <= len - 4.  The OID is not checked against the hash, as in the reference. */
+ECC_HD bool bign_adata_parse(const uint8_t *ad, uint64_t len, uint32_t &oid_len, uint32_t &t_len)
+{
+	oid_len = t_len = 0;
+	if (len < 4 || len > kBignMaxAdata) return false;
+	oid_len = (uint32_t)ad[0] << 8 | ad[1];
+	t_len = (uint32_t)ad[2] << 8 | ad[3];
+	return oid_len + t_len <= len - 4;
+}
+
+/* len little-endian bytes -> N words */
+template <int N> ECC_HD void load_le(Fe<N> &r, const uint8_t *buf, int len)
+{
+	for (int i = 0; i < N; i++) r.w[i] = 0;
+	for (int j = 0; j < len && j < 4 * N; j++) r.w[j >> 2] |= (uint32_t)buf[j] << (8 * (j & 3));
+}
+
+/* a < b on N-word integers */
+template <int N> ECC_HD bool fe_less(const Fe<N> &a, const Fe<N> &b)
+{
+	uint32_t borrow = 0;
+#pragma unroll
+	for (int i = 0; i < N; i++) {
+		const uint64_t t = (uint64_t)a.w[i] - b.w[i] - borrow;
+		borrow = (uint32_t)(t >> 32) & 1u;
+	}
+	return borrow != 0;
+}
+
+/*
+ * s0 = the first min(l, 32) bytes of BELT-HASH(oid || the first 2l bytes of LE(W_x) || h), zero-padded to l bytes,
+ * l = qlen / 2 (step 4 of __bign_sign_finalize, sig/bign_common.c:626-645; step 6 of __bign_verify_finalize,
+ * :939-957).  2l <= plen on every curve, so W_y never enters.  W is the affine wire point, h the hs-byte digest H(m);
+ * the concatenation is the three-segment source, never built in memory.
+ */
+template <class C>
+ECC_D void bign_s0(uint8_t *s0, const uint8_t *oid, uint32_t oid_len, const uint8_t *W, const uint8_t *h, int hs,
+		   const uint8_t *H)
+{
+	constexpr int L = C::QLEN / 2, PL = C::PLEN;
+	static_assert(2 * L <= PL, "bign_s0: 2l bytes of W_x");
+	uint8_t wle[2 * L], d[32];
+	for (int i = 0; i < 2 * L; i++) wle[i] = W[PL - 1 - i];
+	belt_hash_src(Seg3{ oid, oid_len, wle, (uint64_t)(2 * L), h }, (uint64_t)oid_len + 2 * L + (uint64_t)hs, d, H);
+	for (int i = 0; i < L; i++) s0[i] = i < 32 ? d[i] : 0u;
+}
+
+/* h-bar = OS2I(byte-reversed h) mod q over the whole digest (:650-652 sign, :913-915 verify); rev: 64 bytes */
+template <class C> ECC_HD void bign_digest_scalar(Fe<C::N> &e, const uint8_t *h, int hs, uint8_t *rev)
+{
+	for (int i = 0; i < hs; i++) rev[i] = h[hs - 1 - i];
+	digest_full_mod_q<C>(e, rev, (uint32_t)hs);
+}
+
+/* s0-bar + 2^(8l) from the l-byte s0.  s0-bar < 2^(8l) and 2^(8l+1) < q on every curve, so the sum is already
+ * reduced, never 0, and 2^(8l) mod q is the constant bit 8l (:659-663 sign, :924-928 verify). */
+template <class C> ECC_HD void bign_s0_scalar(Fe<C::N> &b, const uint8_t *s0)
+{
+	constexpr int L = C::QLEN / 2;
+	static_assert(8 * L + 1 < C::QBITS, "bign: 2^(8l+1) < q");
+	load_le<C::N>(b, s0, L);
+	b.w[(8 * L) / 32] |= 1u << ((8 * L) % 32);
+}
+
+/*
+ * DBIGN's nonce (__bign_determinitic_nonce, sig/bign_common.c:200-342; STB 34.101.45 §6.3.3) from the key
+ * theta = BELT-HASH(oid || first 2l bytes of LE(x) || t) and the hlen-byte digest h, for the group order q of qbits
+ * bits (arguments, so that the host tests can run it on the STB curves):
+ *   r = h zero-padded to n = max(2, hlen / 16) blocks r_1 .. r_n;  for i = 1, 2, ...:
+ *     s = r_1 ^ .. ^ r_{n-1};  r <- r_2 .. r_{n-1} || belt-block(s, theta) ^ r_n ^ <i>_128 || s;
+ *     k = the first qlen bytes of r read little-endian, masked to qbits bits (all 16n bytes, unmasked, when
+ *     qlen >= 16n: SECP521R1 with a digest of 64 bytes or fewer);
+ *   until i >= 2n and 0 < k < q.  Returns the number of rounds.
+ */
+template <int N>
+ECC_HD uint32_t bign_det_nonce(Fe<N> &k, const uint8_t *theta, const uint8_t *h, int hlen, const Fe<N> &q, int qbits,
+			       const uint8_t *H)
+{
+	uint32_t key[8], r[4][4];
+	belt_load_block(key, theta);
+	belt_load_block(key + 4, theta + 16);
+	const int n = hlen / 16 > 2 ? hlen / 16 : 2, qlen = (qbits + 7) / 8;
+	const bool whole = qlen >= 16 * n;
+#pragma unroll
+	for (int j = 0; j < 4; j++) {
+		uint8_t blk[16];
+		for (int z = 0; z < 16; z++) blk[z] = 16 * j + z < hlen ? h[16 * j + z] : 0u;
+		belt_load_block(r[j], blk);
+	}
+	for (uint32_t i = 1;; i++) {
+		uint32_t s[4] = { 0, 0, 0, 0 }, e[4];
+#pragma unroll
+		for (int j = 0; j < 3; j++)
+			if (j < n - 1)
+				for (int w = 0; w < 4; w++) s[w] ^= r[j][w];
+		for (int w = 0; w < 4; w++) e[w] = s[w];
+		belt_block(e, key, H);
+		e[0] ^= i;
+#pragma unroll
+		for (int j = 0; j < 4; j++) {
+			if (j + 1 < n)
+				for (int w = 0; w < 4; w++) r[j][w] = r[j + 1][w] ^ (j + 2 == n ? e[w] : 0u);
+			else if (j + 1 == n)
+				for (int w = 0; w < 4; w++) r[j][w] = s[w];
+		}
+#pragma unroll
+		for (int m = 0; m < N; m++) {
+			uint32_t v = m < 16 && m < 4 * n ? r[(m >> 2) & 3][m & 3] : 0u;
+			if (!whole) {
+				const int lo = 32 * m;
+				v = lo >= qbits ? 0u : (qbits - lo >= 32 ? v : v & ((1u << (qbits - lo)) - 1u));
+			}
+			k.w[m] = v;
+		}
+		bool zero = true;
+#pragma unroll
+		for (int m = 0; m < N; m++) zero = zero && k.w[m] == 0;
+		if (i >= (uint32_t)(2 * n) && !zero && fe_less<N>(k, q)) return i;
+	}
+}
+
+/* theta of bign_det_nonce: BELT-HASH(oid || first 2l bytes of LE(x) || t) (:233-248), x the plain private scalar */
+template <class C>
+ECC_D void bign_theta(uint8_t *theta, const uint8_t *oid, uint32_t oid_len, const uint8_t *t, uint32_t t_len,
+		      const Fe<C::N> &x, const uint8_t *H)
+{
+	constexpr int L = C::QLEN / 2;
+	uint8_t xle[2 * L];
+	for (int i = 0; i < 2 * L; i++) xle[i] = (uint8_t)(x.w[i >> 2] >> (8 * (i & 3)));
+	belt_hash_src(Seg3{ oid, oid_len, xle, (uint64_t)(2 * L), t }, (uint64_t)oid_len + 2 * L + t_len, theta, H);
+}
+
+/* The group order q of the curve as N words */
+template <class C> ECC_HD void bign_order(Fe<C::N> &q)
+{
+#pragma unroll
+	for (int i = 0; i < C::N; i++) q.w[i] = C::Fq::P(i);
+}
+
+/*
+ * One BIGN signature s0 || LE(s1) (l + qlen bytes) from W = k*G (affine wire bytes), the plain scalars x and k, the
+ * digest h = H(m) and the adata record (__bign_sign_finalize steps 4-5, sig/bign_common.c:626-690):
+ *   s1 = (k - h-bar - (s0-bar + 2^(8l)) * x) mod q.
+ * There is no restart case: s1 = 0 is a signature the verifier accepts.  Returns 0, or -1 (sig zeroed) for x or k
+ * outside [1, q-1] or a malformed adata record.
+ */
+template <class C>
+ECC_D int bign_sign_core(uint8_t *sig, const uint8_t *W, const Fe<C::N> &x, const Fe<C::N> &k, const uint8_t *h,
+			 int hs, const uint8_t *ad, uint64_t adlen, const uint8_t *H)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, QL = C::QLEN, L = C::QLEN / 2;
+	uint32_t oid_len, t_len;
+	if (!bign_adata_parse(ad, adlen, oid_len, t_len) || Fq::is_zero(x) || Fq::geq_mod(x) || Fq::is_zero(k) ||
+	    Fq::geq_mod(k)) {
+		for (int i = 0; i < L + QL; i++) sig[i] = 0;
+		return -1;
+	}
+	bign_s0<C>(sig, ad + 4, oid_len, W, h, hs, H);
+	uint8_t rev[64];
+	Fe<N> hb, b, xm, t, s1;
+	bign_digest_scalar<C>(hb, h, hs, rev);
+	bign_s0_scalar<C>(b, sig);
+	Fq::to_mont(xm, x);
+	Fq::mul(t, b, xm); /* (s0-bar + 2^(8l)) * x */
+	Fq::sub(s1, k, hb);
+	Fq::sub(s1, s1, t);
+	for (int i = 0; i < QL; i++) sig[L + i] = (uint8_t)(s1.w[i >> 2] >> (8 * (i & 3)));
+	return 0;
+}
+
+/*
+ * First half of a BIGN verification (__bign_verify_init / __bign_verify_finalize, sig/bign_common.c:742-936): from the
+ * signature s0 || LE(s1) and the digest h, the scalars a = (s1 + h-bar) mod q and b = s0-bar + 2^(8l) of
+ * W' = a*G + b*Y.  False (a = b = 0) for s1 >= q or a malformed adata record.
+ */
+template <class C>
+ECC_HD bool bign_verify_prep_core(Fe<C::N> &a, Fe<C::N> &b, const uint8_t *sig, const uint8_t *h, int hs,
+				  const uint8_t *ad, uint64_t adlen)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N, QL = C::QLEN, L = C::QLEN / 2;
+	uint32_t oid_len, t_len;
+	Fe<N> s1;
+	load_le<N>(s1, sig + L, QL);
+	Fq::set_zero(a);
+	Fq::set_zero(b);
+	if (!bign_adata_parse(ad, adlen, oid_len, t_len) || Fq::geq_mod(s1)) return false;
+	uint8_t rev[64];
+	Fe<N> hb;
+	bign_digest_scalar<C>(hb, h, hs, rev);
+	Fq::add(a, s1, hb);
+	bign_s0_scalar<C>(b, sig);
+	return true;
 }
 
 } // namespace eccb200

@@ -87,8 +87,9 @@ struct eccb200_ctx {
 	uint8_t *unique_io = nullptr; /* device buffer of eccb200_prj_pt_unique_batch (in || out || status), grown on demand:
 	                               * a cudaMalloc / cudaFree pair per call cost up to a second on a busy allocator */
 	size_t unique_io_bytes = 0;
-	uint8_t *sign_k = nullptr; /* [sign_k_cap][qlen] scratch of the device-pointer signers, grown on demand: BIP0340 and
-	                            * RFC 6979 nonces, and the digests of the ECDSA message signer after them */
+	uint8_t *sign_k = nullptr; /* [sign_k_cap][qlen] scratch of the device-pointer signers, grown on demand: BIP0340, RFC 6979
+	                            * and DBIGN nonces, and the digests of the ECDSA and BIGN message signers and of the BIGN
+	                            * verifier after them */
 	size_t sign_k_cap = 0;
 	/* optional per-kernel timing of the device-pointer API (bench.py's roofline leg) */
 	bool profiling = false;
@@ -2093,6 +2094,166 @@ extern "C" int eccb200_ecdsa_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int
 								    ch.sigs, ch.status, ctx->stage_jac[s],
 								    ctx->stage_prefix[s], ctx->stage_aff[s], ctx->streams[s]);
 				  });
+}
+
+/* ------------------------------------------------------------------------------- BIGN / DBIGN of raw messages */
+
+static const char *kBignHashMsg = "unsupported hash (SHA224 = 1, SHA256 = 2, SHA384 = 3, SHA512 = 4, SHA3_224..512 = "
+				  "5..8, SM3 = 11, BELT_HASH = 16, BASH224..512 = 17..20)";
+
+/* k_bign_nonce (H(m) into dig_buf; the DBIGN k into k_buf when det), K1 on k (k_buf, or the caller's d_nonce), K4,
+ * k_bign_sign_finish — all on `st` */
+static int bign_sign_dev(eccb200_ctx *ctx, bool det, int hash_type, uint32_t n, const uint8_t *d_priv,
+			 const uint8_t *d_nonce, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_ad,
+			 const uint64_t *d_ad_off, uint8_t *k_buf, uint8_t *dig_buf, uint8_t *d_sigs, int8_t *d_status,
+			 uint32_t *jac, uint32_t *prefix, uint8_t *aff, cudaStream_t st)
+{
+	if (n == 0) return 0;
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		const uint8_t *k = det ? k_buf : d_nonce;
+		LaunchMisc<C>::bign_nonce(n, hash_type, d_priv, d_msgs, d_off, d_ad, d_ad_off, dig_buf, det ? k_buf : nullptr,
+					  st);                                                    /* H(m), k  */
+		LaunchFixed<C>::fixed(n, k, ctx->table, ctx->w, jac, d_status, st);             /* W = k*G  */
+		LaunchMisc<C>::to_affine(affine_grid(ctx, n), n, jac, prefix, aff, d_status, st); /* affine W */
+		LaunchMisc<C>::bign_sign_finish(n, hash_type, d_priv, k, dig_buf, d_ad, d_ad_off, aff, d_sigs, d_status,
+						st);                                              /* s0, s1   */
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 4;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+/* the checks both signing forms share; 0, or -1 with the reason in eccb200_last_error */
+static int bign_sign_args(const eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n, const void *privkeys,
+			  const void *nonces, const void *offsets, const void *adata, const void *adata_offsets,
+			  const void *sigs, const void *status)
+{
+	if (!ctx) return fail("null argument");
+	if (sig_type != SIG_BIGN && sig_type != SIG_DBIGN) return fail("unsupported sig_type (BIGN = 18, DBIGN = 19)");
+	if (!bign_hash_digest_size(hash_type)) return fail(kBignHashMsg);
+	if (sig_type == SIG_BIGN && !nonces) return fail("BIGN needs the caller's nonces");
+	if (n && (!privkeys || !offsets || !adata || !adata_offsets || !sigs || !status)) return fail("null argument");
+	return 0;
+}
+
+/* Scratch of the signers, per chunk of cnt items: the DBIGN nonces (cnt * qlen bytes), then the digests (cnt * digest
+ * size bytes). */
+extern "C" int eccb200_bign_sign_msgs_batch_dev(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+						const uint8_t *d_privkeys, const uint8_t *d_nonces, const uint8_t *d_msgs,
+						const uint64_t *d_offsets, const uint8_t *d_adata,
+						const uint64_t *d_adata_offsets, uint8_t *d_sigs, int8_t *d_status, void *stream)
+{
+	if (bign_sign_args(ctx, sig_type, hash_type, n, d_privkeys, d_nonces, d_offsets, d_adata, d_adata_offsets, d_sigs,
+			   d_status))
+		return -1;
+	const bool det = sig_type == SIG_DBIGN;
+	if (misaligned16(ctx, { d_privkeys, det ? nullptr : d_nonces, d_sigs })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	const size_t ql = ctx->qlen, ds = (size_t)bign_hash_digest_size(hash_type);
+	const size_t k_bytes = det ? (size_t)n * ql : 0;
+	if (ensure_work(ctx, n) || ensure_sign_k(ctx, (k_bytes + (size_t)n * ds + ql - 1) / ql)) return -1;
+	return bign_sign_dev(ctx, det, hash_type, n, d_privkeys, det ? nullptr : d_nonces, d_msgs, d_offsets, d_adata,
+			     d_adata_offsets, det ? ctx->sign_k : nullptr, ctx->sign_k + k_bytes, d_sigs, d_status, ctx->jac,
+			     ctx->prefix, ctx->aff, (cudaStream_t)stream);
+}
+
+extern "C" int eccb200_bign_sign_msgs_batch(eccb200_ctx *ctx, int sig_type, int hash_type, uint32_t n,
+					    const uint8_t *privkeys, const uint8_t *nonces, const uint8_t *msgs,
+					    const uint64_t *offsets, const uint8_t *adata, const uint64_t *adata_offsets,
+					    uint8_t *sigs, int8_t *status)
+{
+	if (bign_sign_args(ctx, sig_type, hash_type, n, privkeys, nonces, offsets, adata, adata_offsets, sigs, status))
+		return -1;
+	if (n == 0) return 0;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	if (!offsets_ok(adata_offsets, n)) return fail("adata_offsets must start at 0 and be non-decreasing");
+	const bool det = sig_type == SIG_DBIGN;
+	const size_t ql = ctx->qlen, ds = (size_t)bign_hash_digest_size(hash_type);
+	const SignCol cols[3] = { { privkeys, ql }, { det ? nullptr : nonces, ql }, { nullptr, 0 } };
+	const SignRagged rag[2] = { { msgs, offsets }, { adata, adata_offsets } };
+	return sign_msgs_pipeline(ctx, n, cols, (det ? ql : 0) + ds, rag, ql / 2 + ql, sigs, status,
+				  [&](int s, uint32_t cnt, const SignChunk &ch) {
+					  const size_t k_bytes = det ? (size_t)cnt * ql : 0;
+					  return bign_sign_dev(ctx, det, hash_type, cnt, ch.col[0], ch.col[1], ch.rag_base[0],
+							       ch.rag_off[0], ch.rag_base[1], ch.rag_off[1],
+							       det ? ch.scratch : nullptr, ch.scratch + k_bytes, ch.sigs,
+							       ch.status, ctx->stage_jac[s], ctx->stage_prefix[s],
+							       ctx->stage_aff[s], ctx->streams[s]);
+				  });
+}
+
+/* k_bign_verify_prep (checks, H(m) into dig_buf, a || b into jac), the double-scalar kernel (W' into aff, its status
+ * into d_verdict), k_bign_verify_finish (s0 test) — all on `st` */
+static int bign_verify_dev(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *d_sigs, const uint8_t *d_pub,
+			   const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_ad, const uint64_t *d_ad_off,
+			   uint8_t *dig_buf, int8_t *d_verdict, uint32_t *jac, uint8_t *aff, cudaStream_t st)
+{
+	if (n == 0) return 0;
+	const int ds = bign_hash_digest_size(hash_type);
+	return dispatch(ctx->curve_id, [&](auto c) {
+		typedef decltype(c) C;
+		static_assert(2 * C::QLEN <= 12 * C::N, "verify scratch layout"); /* [n][2*qlen] bytes in [n][3N] words */
+		uint8_t *ab = reinterpret_cast<uint8_t *>(jac);
+		if (jac == ctx->jac) scratch_enter(ctx, st);
+		LaunchMisc<C>::bign_verify_prep(n, hash_type, d_sigs, d_msgs, d_off, d_ad, d_ad_off, dig_buf, ab, st);
+		LaunchVerify<C>::double_smul(n, ab, d_pub, ctx->table, ctx->w, aff, d_verdict, st); /* W' = aG + bY */
+		LaunchMisc<C>::bign_verify_finish(n, d_sigs, d_ad, d_ad_off, dig_buf, ds, aff, d_verdict, st);
+		if (jac == ctx->jac) scratch_leave(ctx, st);
+		ctx->launches += 3;
+		CUDA_OK(cudaGetLastError());
+		return 0;
+	});
+}
+
+static int bign_verify_args(const eccb200_ctx *ctx, int hash_type, uint32_t n, const void *sigs, const void *pubkeys,
+			    const void *offsets, const void *adata, const void *adata_offsets, const void *verdict)
+{
+	if (!ctx) return fail("null argument");
+	if (!bign_hash_digest_size(hash_type)) return fail(kBignHashMsg);
+	if (n && (!sigs || !pubkeys || !offsets || !adata || !adata_offsets || !verdict)) return fail("null argument");
+	return 0;
+}
+
+extern "C" int eccb200_bign_verify_msgs_batch_dev(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *d_sigs,
+						  const uint8_t *d_pubkeys, const uint8_t *d_msgs, const uint64_t *d_offsets,
+						  const uint8_t *d_adata, const uint64_t *d_adata_offsets, int8_t *d_verdict,
+						  void *stream)
+{
+	if (bign_verify_args(ctx, hash_type, n, d_sigs, d_pubkeys, d_offsets, d_adata, d_adata_offsets, d_verdict))
+		return -1;
+	if (misaligned16(ctx, { d_sigs, d_pubkeys })) return fail(kAlignMsg);
+	if (n == 0) return 0;
+	CUDA_OK(cudaSetDevice(ctx->device));
+	const size_t ql = ctx->qlen, ds = (size_t)bign_hash_digest_size(hash_type);
+	if (ensure_work(ctx, n) || ensure_sign_k(ctx, ((size_t)n * ds + ql - 1) / ql)) return -1;
+	return bign_verify_dev(ctx, hash_type, n, d_sigs, d_pubkeys, d_msgs, d_offsets, d_adata, d_adata_offsets,
+			       ctx->sign_k, d_verdict, ctx->jac, ctx->aff, (cudaStream_t)stream);
+}
+
+/* Host-pointer form through sign_msgs_pipeline: signatures and keys are its columns, messages and adata its ragged
+ * inputs, the digests its scratch column, the verdicts its status column. */
+extern "C" int eccb200_bign_verify_msgs_batch(eccb200_ctx *ctx, int hash_type, uint32_t n, const uint8_t *sigs,
+					      const uint8_t *pubkeys, const uint8_t *msgs, const uint64_t *offsets,
+					      const uint8_t *adata, const uint64_t *adata_offsets, int8_t *verdict)
+{
+	if (bign_verify_args(ctx, hash_type, n, sigs, pubkeys, offsets, adata, adata_offsets, verdict)) return -1;
+	if (n == 0) return 0;
+	if (!offsets_ok(offsets, n)) return fail("offsets must start at 0 and be non-decreasing");
+	if (offsets[n] && !msgs) return fail("null argument");
+	if (!offsets_ok(adata_offsets, n)) return fail("adata_offsets must start at 0 and be non-decreasing");
+	const size_t ql = ctx->qlen, ds = (size_t)bign_hash_digest_size(hash_type);
+	const SignCol cols[3] = { { sigs, ql / 2 + ql }, { pubkeys, 2 * (size_t)ctx->plen }, { nullptr, 0 } };
+	const SignRagged rag[2] = { { msgs, offsets }, { adata, adata_offsets } };
+	return sign_msgs_pipeline(ctx, n, cols, ds, rag, 0, nullptr, verdict, [&](int s, uint32_t cnt, const SignChunk &ch) {
+		return bign_verify_dev(ctx, hash_type, cnt, ch.col[0], ch.col[1], ch.rag_base[0], ch.rag_off[0],
+				       ch.rag_base[1], ch.rag_off[1], ch.scratch, ch.status, ctx->stage_jac[s],
+				       ctx->stage_aff[s], ctx->streams[s]);
+	});
 }
 
 /* -------------------------------------------- ECKCDSA / ECSDSA / ECOSDSA / ECGDSA / ECRDSA / SM2 verification */

@@ -1376,6 +1376,122 @@ __global__ void __launch_bounds__(128) k_msgs_verify_finish(uint32_t n, int sig_
 	verdict[e] = ok ? 0 : -1;
 }
 
+/* ------------------------------------------------------------------------------------- BIGN / DBIGN sign and verify */
+
+/*
+ * Before K1 of the BIGN signers, one item per thread: H(m) into dig_out ([n][digest size]; message i is
+ * msgs[off[i] .. off[i+1]), as k_sha2_batch).  With k_out (DBIGN): the nonce of bign_det_nonce, keyed by the
+ * BELT-HASH of the OID, x and t of item i's adata record (ad[ad_off[i] .. ad_off[i+1])), into k_out; 0 without any
+ * BELT work where x is outside [1, q-1] or the record is malformed (k_bign_sign_finish then reports ECCB200_ERR).
+ */
+template <class C>
+__global__ void __launch_bounds__(128) k_bign_nonce(uint32_t n, int hash_type, const uint8_t *__restrict__ privkeys,
+						    const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+						    const uint8_t *__restrict__ ad, const uint64_t *__restrict__ ad_off,
+						    uint8_t *__restrict__ dig_out, uint8_t *__restrict__ k_out)
+{
+	typedef Field<typename C::Fq> Fq;
+	constexpr int N = C::N;
+	__shared__ uint8_t sbox[256];
+	belt_sbox_to_shared(sbox);
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	const int ds = bign_hash_digest_size(hash_type);
+	uint8_t h[64];
+	bign_hash_src(hash_type, ByteSpan{ msgs + off[idx] }, off[idx + 1] - off[idx], h, sbox);
+	for (int i = 0; i < ds; i++) dig_out[(size_t)idx * ds + i] = h[i];
+	if (!k_out) return;
+	Fe<N> x, k;
+	load_wire<N, C::QLEN>(x, privkeys + (size_t)idx * C::QLEN);
+	Fq::set_zero(k);
+	const uint8_t *rec = ad + ad_off[idx];
+	uint32_t oid_len, t_len;
+	if (!Fq::is_zero(x) && !Fq::geq_mod(x) && bign_adata_parse(rec, ad_off[idx + 1] - ad_off[idx], oid_len, t_len)) {
+		uint8_t theta[32];
+		Fe<N> q;
+		bign_theta<C>(theta, rec + 4, oid_len, rec + 4 + oid_len, t_len, x, sbox);
+		bign_order<C>(q);
+		bign_det_nonce<N>(k, theta, h, ds, q, C::QBITS, sbox);
+	}
+	store_wire<N, C::QLEN>(k_out + (size_t)idx * C::QLEN, k);
+}
+
+/* After K1 (k*G) and K4 (affine W), one item per thread: s0 || LE(s1) (bign_sign_core) from the digest column.
+ * sigs: [n][l + qlen], status: 0 / -1 (ECCB200_OK / _ERR). */
+template <class C>
+__global__ void __launch_bounds__(128) k_bign_sign_finish(uint32_t n, int hash_type,
+							  const uint8_t *__restrict__ privkeys,
+							  const uint8_t *__restrict__ nonces,
+							  const uint8_t *__restrict__ digests, const uint8_t *__restrict__ ad,
+							  const uint64_t *__restrict__ ad_off, const uint8_t *__restrict__ W_aff,
+							  uint8_t *__restrict__ sigs, int8_t *__restrict__ status)
+{
+	constexpr int N = C::N, SL = C::QLEN / 2 + C::QLEN;
+	__shared__ uint8_t sbox[256];
+	belt_sbox_to_shared(sbox);
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	const int ds = bign_hash_digest_size(hash_type);
+	Fe<N> x, k;
+	load_wire<N, C::QLEN>(x, privkeys + (size_t)idx * C::QLEN);
+	load_wire<N, C::QLEN>(k, nonces + (size_t)idx * C::QLEN);
+	status[idx] = (int8_t)bign_sign_core<C>(sigs + (size_t)idx * SL, W_aff + (size_t)idx * (2 * C::PLEN), x, k,
+						digests + (size_t)idx * ds, ds, ad + ad_off[idx],
+						ad_off[idx + 1] - ad_off[idx], sbox);
+}
+
+/* First launch of a BIGN verification, one item per thread: H(m) into dig_out, and a || b of W' = a*G + b*Y
+ * (bign_verify_prep_core) into ab ([n][2*qlen]); a rejected item gets a = b = 0, which the double-scalar kernel turns
+ * into infinity (status 1).  b is never 0 otherwise, so a valid item never reaches infinity. */
+template <class C>
+__global__ void __launch_bounds__(128) k_bign_verify_prep(uint32_t n, int hash_type, const uint8_t *__restrict__ sigs,
+							  const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off,
+							  const uint8_t *__restrict__ ad, const uint64_t *__restrict__ ad_off,
+							  uint8_t *__restrict__ dig_out, uint8_t *__restrict__ ab)
+{
+	constexpr int N = C::N, QL = C::QLEN, SL = C::QLEN / 2 + C::QLEN;
+	__shared__ uint8_t sbox[256];
+	belt_sbox_to_shared(sbox);
+	const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= n) return;
+	const int ds = bign_hash_digest_size(hash_type);
+	uint8_t h[64];
+	bign_hash_src(hash_type, ByteSpan{ msgs + off[idx] }, off[idx + 1] - off[idx], h, sbox);
+	for (int i = 0; i < ds; i++) dig_out[(size_t)idx * ds + i] = h[i];
+	Fe<N> a, b;
+	bign_verify_prep_core<C>(a, b, sigs + (size_t)idx * SL, h, ds, ad + ad_off[idx], ad_off[idx + 1] - ad_off[idx]);
+	store_wire<N, QL>(ab + (size_t)idx * (2 * QL), a);
+	store_wire<N, QL>(ab + (size_t)idx * (2 * QL) + QL, b);
+}
+
+/* Last launch, one item per thread: verdict holds the double-scalar kernel's status (0 W' finite, 1 infinity, -1 key
+ * off the curve), W_aff the affine W'.  Status 0, a well-formed adata record and s0 == the first l bytes of
+ * BELT-HASH(oid || LE(W'_x) || h) (bign_s0) give 0; anything else gives -1. */
+template <class C>
+__global__ void __launch_bounds__(128) k_bign_verify_finish(uint32_t n, const uint8_t *__restrict__ sigs,
+							    const uint8_t *__restrict__ ad, const uint64_t *__restrict__ ad_off,
+							    const uint8_t *__restrict__ digests, int ds,
+							    const uint8_t *__restrict__ W_aff, int8_t *__restrict__ verdict)
+{
+	constexpr int L = C::QLEN / 2, SL = C::QLEN / 2 + C::QLEN;
+	__shared__ uint8_t sbox[256];
+	belt_sbox_to_shared(sbox);
+	const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+	if (e >= n) return;
+	const uint8_t *rec = ad + ad_off[e];
+	uint32_t oid_len, t_len;
+	bool ok = verdict[e] == 0 && bign_adata_parse(rec, ad_off[e + 1] - ad_off[e], oid_len, t_len);
+	if (ok) {
+		uint8_t s0[L];
+		bign_s0<C>(s0, rec + 4, oid_len, W_aff + (size_t)e * (2 * C::PLEN), digests + (size_t)e * ds, ds, sbox);
+		const uint8_t *sig = sigs + (size_t)e * SL;
+		uint8_t diff = 0;
+		for (int i = 0; i < L; i++) diff |= s0[i] ^ sig[i];
+		ok = diff == 0;
+	}
+	verdict[e] = ok ? 0 : -1;
+}
+
 /* ------------------------------------------------------------------------------------------ Schnorr-family sign */
 
 /* H(tag) of BIP0340 tags tag0 .. tag0 + ntags - 1 into shared memory, one thread per tag: once per CTA, not per item */
@@ -1682,6 +1798,15 @@ template <class C> struct LaunchMisc {
 	static void msgs_verify_finish(uint32_t n, int sig_type, int hash_type, const uint8_t *sigs, const uint8_t *pubkeys,
 				       const uint8_t *msgs, const uint64_t *off, const uint8_t *ids, const uint64_t *id_off,
 				       const uint8_t *W_aff, int8_t *verdict, cudaStream_t st);
+	static void bign_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *msgs, const uint64_t *off,
+			       const uint8_t *ad, const uint64_t *ad_off, uint8_t *dig_out, uint8_t *k_out, cudaStream_t st);
+	static void bign_sign_finish(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *nonces,
+				     const uint8_t *digests, const uint8_t *ad, const uint64_t *ad_off, const uint8_t *W_aff,
+				     uint8_t *sigs, int8_t *status, cudaStream_t st);
+	static void bign_verify_prep(uint32_t n, int hash_type, const uint8_t *sigs, const uint8_t *msgs, const uint64_t *off,
+				     const uint8_t *ad, const uint64_t *ad_off, uint8_t *dig_out, uint8_t *ab, cudaStream_t st);
+	static void bign_verify_finish(uint32_t n, const uint8_t *sigs, const uint8_t *ad, const uint64_t *ad_off,
+				       const uint8_t *digests, int ds, const uint8_t *W_aff, int8_t *verdict, cudaStream_t st);
 	static void fp_mul(int which, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out, cudaStream_t st);
 	static void fp_addsub(int which, int op, uint32_t n, const uint8_t *a, const uint8_t *b, uint8_t *out,
 			      cudaStream_t st);
@@ -1818,6 +1943,33 @@ void LaunchMisc<C>::msgs_verify_finish(uint32_t n, int sig_type, int hash_type, 
 {
 	k_msgs_verify_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, sig_type, hash_type, sigs, pubkeys, msgs, off, ids,
 								   id_off, W_aff, verdict);
+}
+template <class C>
+void LaunchMisc<C>::bign_nonce(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *msgs, const uint64_t *off,
+			       const uint8_t *ad, const uint64_t *ad_off, uint8_t *dig_out, uint8_t *k_out, cudaStream_t st)
+{
+	k_bign_nonce<C><<<grid_for(n), kThreads, 0, st>>>(n, hash_type, privkeys, msgs, off, ad, ad_off, dig_out, k_out);
+}
+template <class C>
+void LaunchMisc<C>::bign_sign_finish(uint32_t n, int hash_type, const uint8_t *privkeys, const uint8_t *nonces,
+				     const uint8_t *digests, const uint8_t *ad, const uint64_t *ad_off, const uint8_t *W_aff,
+				     uint8_t *sigs, int8_t *status, cudaStream_t st)
+{
+	k_bign_sign_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, hash_type, privkeys, nonces, digests, ad, ad_off, W_aff,
+								 sigs, status);
+}
+template <class C>
+void LaunchMisc<C>::bign_verify_prep(uint32_t n, int hash_type, const uint8_t *sigs, const uint8_t *msgs,
+				     const uint64_t *off, const uint8_t *ad, const uint64_t *ad_off, uint8_t *dig_out,
+				     uint8_t *ab, cudaStream_t st)
+{
+	k_bign_verify_prep<C><<<grid_for(n), kThreads, 0, st>>>(n, hash_type, sigs, msgs, off, ad, ad_off, dig_out, ab);
+}
+template <class C>
+void LaunchMisc<C>::bign_verify_finish(uint32_t n, const uint8_t *sigs, const uint8_t *ad, const uint64_t *ad_off,
+				       const uint8_t *digests, int ds, const uint8_t *W_aff, int8_t *verdict, cudaStream_t st)
+{
+	k_bign_verify_finish<C><<<grid_for(n), kThreads, 0, st>>>(n, sigs, ad, ad_off, digests, ds, W_aff, verdict);
 }
 template <class C>
 void LaunchMisc<C>::prj_unique(uint32_t blocks, uint32_t n, const uint8_t *prj, uint32_t *jac, uint32_t *prefix,
